@@ -312,6 +312,18 @@ int pxr_ba_debug_linearize(pxr_ba* ba, double radius, double* cost, double* Hcc,
 /* Runs the per-point inner iterations (ceres CoordinateDescentMinimizer equivalent) once on the
  * current parameters (parity tests). */
 int pxr_ba_debug_inner_iterations(pxr_ba* ba);
+/* K0 + K1 (Jacobian mode) at the current parameters over the observations list[0..n), the evaluation one batched
+ * inner-iteration round runs (tests).  out [n_obs][8]: s, g^T r (2), g^T g (3 uniques), 0, 0 of every listed
+ * observation, NaN elsewhere.  count_on_device = 1 passes n (at most n_obs) through device memory, grids sized for
+ * all observations. */
+int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count_on_device, double* out);
+/* The rounds of the most recent batched inner iterations (profiling).  *n_rounds = rounds run; for the first
+ * min(*n_rounds, capacity) of them counts[2r] = active observations, counts[2r+1] = active points, and ms[r] = the
+ * round's stream time (events around its launches, device idle time waiting for the host included) when round timing
+ * was on during that call (else -1).  enable_timing >= 0 switches round timing
+ * on / off for the calls that follow.  Any output may be NULL. */
+int pxr_ba_debug_inner_rounds(pxr_ba* ba, int enable_timing, int capacity, unsigned long long* counts, double* ms,
+                              int* n_rounds);
 /* Timing hooks for bench.py: run `iters` LM iterations' worth of the named stage on the
  * resident problem and return the average device time per launch in ms (CUDA events on the
  * library stream).  stage: 0 residual/Jacobian kernel (K1), 1 cost-only kernel, 2 projection+K1+block build,

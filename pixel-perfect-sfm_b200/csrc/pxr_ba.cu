@@ -30,8 +30,8 @@ static int launch_fm(pxr_ctx* ctx, const FmEvalArgs& a, int* n_partials) {
     PXR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
     attr_set = true;
   }
-  const int64_t n_batches = cdiv(a.end - a.begin, 32);
-  int64_t grid = cdiv(n_batches, Cfg::kWarps);
+  // enough CTAs for one item per warp, up to what is resident: the kernel spreads the items evenly over the warps it gets
+  int64_t grid = cdiv(a.end - a.begin, Cfg::kWarps);
   const int64_t resident = (int64_t)ctx->sm_count * std::max(1, (int)(200 * 1024 / Cfg::kSmem));
   if (grid > resident) grid = resident;
   if (grid < 1) grid = 1;
@@ -962,7 +962,7 @@ int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long l
   pa.corner = corner.p; pa.scale = scale.p; pa.ups = ups;
   pa.obs_begin = 0; pa.obs_end = n; pa.item_index = list; pa.n_dev = n_dev;
   pa.uv = uv.p; pa.xy = nullptr; pa.juv = juv.p; pa.juv_stride = juv_stride; pa.juv_k = K;
-  PXR_LAUNCH(ctx, ba_project_kernel<true>, (unsigned)cdiv(n, 128), 128, 0, pa);
+  PXR_LAUNCH(ctx, ba_project_kernel<true>, (unsigned)std::min<int64_t>(cdiv(n, 128), (int64_t)ctx->sm_count * 16), 128, 0, pa);
   FmEvalArgs a;
   a.uv = uv.p; a.item_patch = obs_patch.p; a.item_ref = obs_pt.p;
   a.patches = d_patches; a.ph = ph; a.pw = pw;
@@ -986,35 +986,63 @@ int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long l
 }
 
 // Inner iterations, batched: see pxr_inner.cuh.  Same state machine as ba_inner_kernel.
-// The rounds are enqueued WITHOUT waiting for the host: the list length of a round stays on the device (K0 / K1 read it
-// there, their grids are sized for all observations), its copy travels to a pinned slot behind an event, and the host
-// stops enqueuing once a round two behind has reported an empty list (the two extra rounds find nothing to do).
+// Round 0's lists come from every variable point; from then on a round is three launches (K0, K1, inner_step_kernel) and
+// the step kernel builds the next round's lists.  Lists alternate between two buffers, counters rotate through three sets
+// (the step kernel of round r appends to set r+1 and zeroes set r+2, which no launch of round r touches).  The rounds are
+// enqueued WITHOUT waiting for the host: each step kernel copies its round's list lengths to a host-mapped slot, tagged
+// with the call's epoch, and the host stops enqueuing once a round two behind has reported an empty list (the two extra
+// rounds find nothing to do).
 constexpr int kInnerRounds = 53;
 int BA::inner_rounds(int set) {
   cudaStream_t s = ctx->stream;
+  volatile unsigned long long* slots = inner_cnt_host;
+  const unsigned long long epoch = ++inner_epoch;
+  auto published = [&](int r) { return slots[3 * r + 2] == epoch; };
   InnerStepArgs a;
   a.n_points = n_points; a.point_off = point_off.p; a.pt_begin = pt_begin.p;
   a.obs_out = obs_out.p; a.juv = juv.p; a.juv_stride = juv_stride; a.juv_w = 9 + K;
   a.xyz = X[set].p; a.st = inner_state.p;
   a.loss.type = opt.loss_type; a.loss.a = opt.loss_scale;
-  a.list = inner_list.p; a.counters = inner_counters.p;
+  a.epoch = epoch;
   const unsigned pgrid = (unsigned)cdiv(n_points, 128);
+  const unsigned sgrid = (unsigned)std::min<int64_t>(pgrid, (int64_t)ctx->sm_count * 8);
+  if (time_inner_rounds && inner_round_timed.empty()) {
+    inner_round_timed.resize(kInnerRounds, {nullptr, nullptr});
+    for (auto& pr : inner_round_timed) { PXR_CUDA(cudaEventCreate(&pr.first)); PXR_CUDA(cudaEventCreate(&pr.second)); }
+  }
+  inner_rounds_timed = time_inner_rounds;
+  inner_rounds_run = 0;
+  PXR_CUDA(cudaMemsetAsync(inner_counters.p, 0, 6 * sizeof(unsigned long long), s));
+  a.plist_next = inner_plist[0].p; a.list_next = inner_list[0].p; a.cnt_next = inner_counters.p;
+  PXR_LAUNCH(ctx, inner_list_kernel, pgrid, 128, 0, a);
   for (int round = 0; round < kInnerRounds; ++round) {
     if (round >= 2) {
-      const cudaError_t q = cudaEventQuery(inner_events[round - 2]);
-      if (q == cudaSuccess) { if (inner_cnt_host[2 * (round - 2)] == 0) break; }
-      else if (q != cudaErrorNotReady) PXR_CUDA(q);
-      else if ((void)cudaGetLastError(), round >= 8 && (round & 3) == 0) {        // far ahead of the device: let it catch up rather than pile up empty rounds
-        PXR_CUDA(cudaEventSynchronize(inner_events[round - 2]));
-        if (inner_cnt_host[2 * (round - 2)] == 0) break;
+      const int r2 = round - 2;
+      if (!published(r2) && round >= 8 && (round & 3) == 0) {   // far ahead of the device: let it catch up rather than pile up empty rounds
+        while (!published(r2)) {
+          const cudaError_t q = cudaStreamQuery(s);
+          if (q == cudaSuccess) {
+            if (published(r2)) break;
+            return fail(PXR_ERR_CUDA, "inner iterations: round %d did not report its list", r2);
+          }
+          if (q != cudaErrorNotReady) PXR_CUDA(q);
+          (void)cudaGetLastError();
+          std::this_thread::yield();
+        }
       }
+      if (published(r2) && slots[3 * r2] == 0) break;
     }
-    PXR_CUDA(cudaMemsetAsync(inner_counters.p, 0, 2 * sizeof(unsigned long long), s));
-    PXR_LAUNCH(ctx, inner_list_kernel, pgrid, 128, 0, a, round == 0 ? 1 : 0);
-    PXR_CUDA(cudaMemcpyAsync(inner_cnt_host + 2 * round, inner_counters.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    PXR_CUDA(cudaEventRecord(inner_events[round], s));
-    PXR_TRY(eval_list(set, inner_list.p, n_obs, inner_counters.p, false));
-    PXR_LAUNCH(ctx, inner_step_kernel, pgrid, 128, 0, a, round == 0 ? 0 : 1);
+    const int cur = round & 1;
+    unsigned long long* cnt = inner_counters.p + 2 * (round % 3);
+    a.plist = inner_plist[cur].p; a.cnt = cnt;
+    a.plist_next = inner_plist[1 - cur].p; a.list_next = inner_list[1 - cur].p;
+    a.cnt_next = inner_counters.p + 2 * ((round + 1) % 3); a.cnt_clear = inner_counters.p + 2 * ((round + 2) % 3);
+    a.publish = inner_cnt_dev + 3 * round;
+    if (inner_rounds_timed) PXR_CUDA(cudaEventRecord(inner_round_timed[round].first, s));
+    PXR_TRY(eval_list(set, inner_list[cur].p, n_obs, cnt, false));
+    PXR_LAUNCH(ctx, inner_step_kernel, sgrid, 128, 0, a, round == 0 ? 0 : 1);
+    if (inner_rounds_timed) PXR_CUDA(cudaEventRecord(inner_round_timed[round].second, s));
+    inner_rounds_run = round + 1;
   }
   PXR_CUDA(cudaGetLastError());
   return PXR_OK;
@@ -1026,11 +1054,11 @@ int BA::inner_iterations_batched(int set) {
   cudaStream_t s = ctx->stream;
   if (!inner_state.p) {
     PXR_TRY(inner_state.alloc(n_points));
-    PXR_TRY(inner_list.alloc(n_obs));
-    PXR_TRY(inner_counters.alloc(2));
-    PXR_CUDA(cudaHostAlloc((void**)&inner_cnt_host, (size_t)kInnerRounds * 2 * sizeof(unsigned long long), cudaHostAllocDefault));
-    inner_events.resize(kInnerRounds, nullptr);
-    for (auto& e : inner_events) PXR_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    for (int k = 0; k < 2; ++k) { PXR_TRY(inner_list[k].alloc(n_obs)); PXR_TRY(inner_plist[k].alloc(n_points)); }
+    PXR_TRY(inner_counters.alloc(6));
+    PXR_CUDA(cudaHostAlloc((void**)&inner_cnt_host, (size_t)kInnerRounds * 3 * sizeof(unsigned long long), cudaHostAllocMapped));
+    std::memset(inner_cnt_host, 0, (size_t)kInnerRounds * 3 * sizeof(unsigned long long));
+    PXR_CUDA(cudaHostGetDevicePointer((void**)&inner_cnt_dev, inner_cnt_host, 0));
   }
   if (!resident) return inner_rounds(set);
   // window residency: an observation may leave its window in any round and nobody looks before the rounds are over — keep
@@ -1659,6 +1687,58 @@ int pxr_ba_debug_inner_iterations(pxr_ba* ba) {
   PXR_CUDA(cudaSetDevice(b->ctx->device));
   PXR_TRY(b->inner_iterations(b->cur));
   PXR_CUDA(cudaStreamSynchronize(b->ctx->stream));
+  return PXR_OK;
+}
+
+// K0 + K1 (Jacobian mode) at the current parameters over a list of observations, as one inner-iteration round evaluates
+// them (tests): out [n_obs][8] is the per-observation record, NaN for observations not in the list.  count_on_device = 1
+// passes the list length through device memory with the grids sized for all observations, as the rounds do.
+int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count_on_device, double* out) {
+  if (!ba || n < 0 || (n > 0 && !list) || !out) return fail(PXR_ERR_INVALID_ARGUMENT, "bad arguments");
+  BA* b = reinterpret_cast<BA*>(ba);
+  pxr_ctx* ctx = b->ctx;
+  cudaStream_t s = ctx->stream;
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  if (count_on_device && n > b->n_obs) return fail(PXR_ERR_INVALID_ARGUMENT, "a list counted on the device holds at most n_obs entries");
+  for (int64_t i = 0; i < n; ++i)
+    if (list[i] < 0 || list[i] >= b->n_obs) return fail(PXR_ERR_INVALID_ARGUMENT, "list entry out of range");
+  DevBuf<int64_t> dlist;
+  DevBuf<unsigned long long> dn;
+  if (n > 0) PXR_TRY(dlist.upload(list, (size_t)n, s));
+  PXR_CUDA(cudaMemsetAsync(b->obs_out.p, 0xff, (size_t)b->n_obs * 64, s));
+  if (count_on_device) {
+    const unsigned long long hn = (unsigned long long)n;
+    PXR_TRY(dn.upload(&hn, 1, s));
+    PXR_TRY(b->eval_list(b->cur, dlist.p, b->n_obs, dn.p));
+  } else {
+    PXR_TRY(b->eval_list(b->cur, dlist.p, n));
+  }
+  PXR_CUDA(cudaMemcpyAsync(out, b->obs_out.p, (size_t)b->n_obs * 64, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  return PXR_OK;
+}
+
+// The rounds of the most recent batched inner iterations (profiling): for every round r < *n_rounds (at most `capacity`
+// are written) counts[2r] active observations and counts[2r+1] active points, and ms[r] its stream time if round timing
+// was on during that call (else -1): events around the round's launches, so any time the device waits for the host to
+// enqueue the round's work counts too.  enable_timing >= 0 switches round timing on / off for the calls that follow.
+int pxr_ba_debug_inner_rounds(pxr_ba* ba, int enable_timing, int capacity, unsigned long long* counts, double* ms, int* n_rounds) {
+  if (!ba || capacity < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "bad arguments");
+  BA* b = reinterpret_cast<BA*>(ba);
+  PXR_CUDA(cudaSetDevice(b->ctx->device));
+  PXR_CUDA(cudaStreamSynchronize(b->ctx->stream));
+  const int n = b->inner_cnt_host ? b->inner_rounds_run : 0;
+  if (n_rounds) *n_rounds = n;
+  for (int r = 0; r < std::min(n, capacity); ++r) {
+    if (counts) { counts[2 * r] = b->inner_cnt_host[3 * r]; counts[2 * r + 1] = b->inner_cnt_host[3 * r + 1]; }
+    if (ms) {
+      float t = -1.f;
+      if (b->inner_rounds_timed)
+        PXR_CUDA(cudaEventElapsedTime(&t, b->inner_round_timed[r].first, b->inner_round_timed[r].second));
+      ms[r] = t;
+    }
+  }
+  if (enable_timing >= 0) b->time_inner_rounds = enable_timing != 0;
   return PXR_OK;
 }
 

@@ -179,7 +179,8 @@ struct BA {
   DevBuf<int64_t> io_chunk_begin; int64_t io_n_chunks = 0;
   DevBuf<long long> chol_trace;     // PXR_CHOL_TRACE=<file>: panel-CTA time stamps
   DevBuf<int> chol_sync;            // flags of the persistent tile-DAG Cholesky (pxr_chol.cuh)
-  ~BA() { if (inner_cnt_host) cudaFreeHost(inner_cnt_host); for (auto e : inner_events) cudaEventDestroy(e); if (res_thread.joinable()) res_thread.join(); if (chol_graph_exec) cudaGraphExecDestroy(chol_graph_exec); for (int k = 0; k < kNumStages; ++k) for (auto& pr : timed[k]) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); } }
+  void clear_inner_round_timing() { for (auto& pr : inner_round_timed) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); } inner_round_timed.clear(); }
+  ~BA() { if (inner_cnt_host) cudaFreeHost(inner_cnt_host); clear_inner_round_timing(); if (res_thread.joinable()) res_thread.join(); if (chol_graph_exec) cudaGraphExecDestroy(chol_graph_exec); for (int k = 0; k < kNumStages; ++k) for (auto& pr : timed[k]) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); } }
   // static co-visibility structure for the Schur complement (see ba_schur_pairs_kernel)
   DevBuf<int32_t> sp_px, sp_py, sp_pp;
   DevBuf<int64_t> sp_chunk_begin;
@@ -229,12 +230,17 @@ struct BA {
   int inner_iterations_batched(int set);
   int eval_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev = nullptr, bool settle = true);
   int inner_rounds(int set);                       // the <= 52 rounds of inner_iterations_batched, without a host wait per round
-  unsigned long long* inner_cnt_host = nullptr;    // pinned [kInnerRounds][2]: the rounds' list counts, read back asynchronously
-  std::vector<cudaEvent_t> inner_events;
+  unsigned long long* inner_cnt_host = nullptr;    // pinned, mapped [kInnerRounds][3]: each round's list lengths + the epoch of the call
+  unsigned long long* inner_cnt_dev = nullptr;     // the same slots, device view (written by inner_step_kernel)
+  unsigned long long inner_epoch = 0;              // incremented per inner_rounds call: tells this call's slots from stale ones
+  int inner_rounds_run = 0;                        // rounds enqueued by the most recent inner_rounds (profiling)
+  bool time_inner_rounds = false;                  // pxr_ba_debug_inner_rounds: stream time of every round of the next calls
+  bool inner_rounds_timed = false;                 // the most recent inner_rounds call recorded them
+  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> inner_round_timed;
   DevBuf<double> inner_snapshot;                   // window residency: the points before a batch of rounds (redo after a refetch)
   DevBuf<InnerState> inner_state;
-  DevBuf<int64_t> inner_list;
-  DevBuf<unsigned long long> inner_counters;
+  DevBuf<int64_t> inner_list[2], inner_plist[2];   // a round's observation / point lists, alternating between rounds
+  DevBuf<unsigned long long> inner_counters;       // 3 x [observations, points], rotating
   bool use_monolithic_inner = false;
   int step_norm_between_sets(double* out);
   int lm_begin();

@@ -75,11 +75,12 @@ __device__ __forceinline__ void project_observation(const ProjectArgs& a, int64_
 
 template <bool JAC>
 __global__ void __launch_bounds__(128) ba_project_kernel(ProjectArgs a) {
-  const int64_t k = a.obs_begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t end = a.n_dev ? a.obs_begin + (int64_t)*a.n_dev : a.obs_end;
-  if (k >= end) return;
-  const int64_t o = a.item_index ? a.item_index[k] : k;
-  project_observation<JAC>(a, o, (JAC && a.juv) ? a.juv + o * (int64_t)a.juv_stride : nullptr);
+  // grid-stride: a list whose length lives on the device gets a grid bounded by the SM count, not by its upper bound
+  for (int64_t k = a.obs_begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < end; k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t o = a.item_index ? a.item_index[k] : k;
+    project_observation<JAC>(a, o, (JAC && a.juv) ? a.juv + o * (int64_t)a.juv_stride : nullptr);
+  }
 }
 
 // Full-pass variant (no item list): the 128 records of a CTA are contiguous in `juv`, so they are assembled in shared
@@ -374,16 +375,20 @@ __global__ void __launch_bounds__(FmCfg<T, C>::kWarps * 32, 1) fm_eval_kernel(Fm
   const bool active = lane < ACTIVE;
   const int64_t item_end = a.end_dev ? a.begin + (int64_t)*a.end_dev : a.end;
   const int64_t n_items = item_end - a.begin;
-  const int64_t n_batches = (n_items + 31) / 32;
   const int64_t warp_global = (int64_t)blockIdx.x * kFmWarps + warp;
   const int64_t warps_total = (int64_t)gridDim.x * kFmWarps;
+  // balanced batches: every warp walks at most R = ceil(n / (32 W)) batches of bsz = ceil(n / (W R)) <= 32 consecutive items,
+  // so a short list spreads one or two items over every warp and a long one leaves no partial last wave of 32-item batches
+  const int64_t rounds = n_items > 0 ? (n_items + 32 * warps_total - 1) / (32 * warps_total) : 0;
+  const int bsz = rounds > 0 ? (int)((n_items + warps_total * rounds - 1) / (warps_total * rounds)) : 32;
+  const int64_t n_batches = rounds > 0 ? (n_items + bsz - 1) / bsz : 0;
   uint32_t phase_bits = 0;
   const int64_t patch_bytes = (int64_t)a.ph * a.pw * TAP_BYTES;
   const bool has_ref = a.refs != nullptr;
 
   for (int64_t batch = warp_global; batch < n_batches; batch += warps_total) {
-    const int nvalid = (int)min((int64_t)32, item_end - (a.begin + batch * 32));
-    int64_t o = a.begin + batch * 32 + lane;
+    const int nvalid = (int)min((int64_t)bsz, item_end - (a.begin + batch * bsz));
+    int64_t o = a.begin + batch * bsz + lane;
     if (a.item_index && lane < nvalid) o = a.item_index[o];
     // ---- phase 1: per-lane window geometry, published to the warp through shared memory
     __syncwarp();

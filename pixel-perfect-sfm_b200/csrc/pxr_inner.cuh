@@ -7,8 +7,10 @@
 // (CoordinateDescentMinimizer::Solve builds Minimizer::Options from defaults):
 // max 50 iterations, function_tolerance 1e-6, gradient_tolerance 1e-10,
 // parameter_tolerance 1e-8, Jacobi scaling, monotonic steps, 5 consecutive invalid steps.
-// The point's feature windows are re-read from L2 on every inner evaluation (they were just
-// touched by the trial-cost pass), so this kernel is L2/compute bound, not HBM bound.
+// Every inner evaluation re-reads the point's feature windows.  On a large problem they are not
+// L2-resident (at BASELINE configs[2] one pass over all observations touches about 2 GB of windows
+// against a 50 MB L2), so the first rounds stream them from HBM like any full K1 pass; only the
+// short lists of the late rounds fit in L2.
 #pragma once
 #include "pxr_ba_kernels.cuh"
 #include "pxr_fm_eval.cuh"
@@ -206,8 +208,12 @@ __global__ void __launch_bounds__(128) ba_inner_kernel(InnerArgs a) {
 
 // ---------------------------------------------------------------------------------------------
 // Batched inner iterations: the same per-point Levenberg-Marquardt state machine, but every
-// evaluation of ALL still-active points goes through the hot kernels K0 + K1 (TMA-staged, the
-// windows are L2 resident), and a thread-per-point kernel applies the LM logic between passes.
+// evaluation of ALL still-active points goes through the hot kernels K0 + K1 (TMA-staged; K1
+// spreads even a short list over all its warps), and a thread-per-point kernel applies the LM
+// logic between passes.  A round is three launches: K0 and K1 over the round's observation list,
+// then inner_step_kernel over its point list, which appends the points that stay active and their
+// observations to the next round's (double-buffered) lists.  The list lengths never leave the
+// device except through a host-mapped slot per round that the host's stop rule reads.
 struct InnerState {
   double x[3];        // last accepted point
   double cand[3];     // candidate being evaluated (also written to the parameter set)
@@ -223,8 +229,14 @@ struct InnerStepArgs {
   double* xyz;          // candidate parameter set
   InnerState* st;
   LossParams loss;
-  int64_t* list;        // active observation list (output of the list kernel)
-  unsigned long long* counters;  // [0] #active observations, [1] #active points
+  // a round's lists: the step kernel walks the active points plist[0..cnt[1]) of this round (their observations
+  // list[0..cnt[0]) were just evaluated) and appends the points that stay active, with their observations, to
+  // plist_next / list_next through cnt_next
+  const int64_t* plist; const unsigned long long* cnt;
+  int64_t* plist_next; int64_t* list_next; unsigned long long* cnt_next;
+  unsigned long long* cnt_clear;   // the counters of the round after next: zeroed here (nobody reads them in this round)
+  unsigned long long* publish;     // host-mapped [3]: cnt[0], cnt[1], then `epoch` once both are visible
+  unsigned long long epoch;
 };
 
 __device__ __forceinline__ bool inner_propose(InnerState& s) {
@@ -273,17 +285,16 @@ __device__ __forceinline__ bool inner_propose(InnerState& s) {
 }
 
 // phase 0: state from the evaluation at the start point; phase 1: judge the evaluated candidate
-static __global__ void __launch_bounds__(128) inner_step_kernel(InnerStepArgs a, int phase) {
-  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= a.n_points) return;
+// returns whether point p stays active (proposes another candidate)
+__device__ __forceinline__ bool inner_step_point(const InnerStepArgs& a, int64_t p, int phase) {
   InnerState s = a.st[p];
   if (phase == 0) {
     s.active = (a.point_off[p] >= 0 && a.pt_begin[p + 1] > a.pt_begin[p]) ? 1 : 0;
     s.iter = 0; s.invalid = 0;
-    if (!s.active) { a.st[p] = s; return; }
+    if (!s.active) { a.st[p] = s; return false; }
 #pragma unroll
     for (int k = 0; k < 3; ++k) s.x[k] = a.xyz[3 * p + k];
-  } else if (!s.active) return;
+  } else if (!s.active) return false;
   // cost / J^T J / J^T r of this point at the evaluated location
   double cost = 0, H[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0};
   for (int64_t o = a.pt_begin[p]; o < a.pt_begin[p + 1]; ++o) {
@@ -354,19 +365,38 @@ static __global__ void __launch_bounds__(128) inner_step_kernel(InnerStepArgs a,
     for (int k = 0; k < 3; ++k) a.xyz[3 * p + k] = s.x[k];
   }
   a.st[p] = s;
+  return go;
 }
 
-// compacts the observations of the active points into `list`
-static __global__ void __launch_bounds__(128) inner_list_kernel(InnerStepArgs a, int all_variable) {
+static __global__ void __launch_bounds__(128) inner_step_kernel(InnerStepArgs a, int phase) {
+  const unsigned long long n = a.cnt[1];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    a.cnt_clear[0] = 0; a.cnt_clear[1] = 0;
+    a.publish[0] = a.cnt[0]; a.publish[1] = n;
+    __threadfence_system();
+    *(volatile unsigned long long*)(a.publish + 2) = a.epoch;
+  }
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const int64_t p = a.plist[i];
+    if (!inner_step_point(a, p, phase)) continue;
+    const int64_t ob = a.pt_begin[p], no = a.pt_begin[p + 1] - ob;
+    const unsigned long long base = atomicAdd(&a.cnt_next[0], (unsigned long long)no);
+    a.plist_next[atomicAdd(&a.cnt_next[1], 1ull)] = p;
+    for (int64_t k = 0; k < no; ++k) a.list_next[base + k] = ob + k;
+  }
+}
+
+// round 0's lists: every variable point with observations, and those observations
+static __global__ void __launch_bounds__(128) inner_list_kernel(InnerStepArgs a) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= a.n_points) return;
-  const bool act = all_variable ? (a.point_off[p] >= 0 && a.pt_begin[p + 1] > a.pt_begin[p]) : (a.st[p].active != 0);
-  if (!act) return;
+  if (!(a.point_off[p] >= 0 && a.pt_begin[p + 1] > a.pt_begin[p])) return;
   const int64_t ob = a.pt_begin[p], n = a.pt_begin[p + 1] - ob;
-  const unsigned long long base = atomicAdd(&a.counters[0], (unsigned long long)n);
-  atomicAdd(&a.counters[1], 1ull);
-  for (int64_t i = 0; i < n; ++i) a.list[base + i] = ob + i;
+  const unsigned long long base = atomicAdd(&a.cnt_next[0], (unsigned long long)n);
+  a.plist_next[atomicAdd(&a.cnt_next[1], 1ull)] = p;
+  for (int64_t i = 0; i < n; ++i) a.list_next[base + i] = ob + i;
 }
+
 
 // ||a - b|| over two parameter sets (ambient), for step_norm after inner iterations
 static __global__ void __launch_bounds__(256) diff_norm_kernel(const double* a, const double* b, int64_t n, double* acc, double* part = nullptr) {

@@ -74,6 +74,23 @@ class BAHandle:
     def debug_inner_iterations(self):
         _capi.check(self.lib.pxr_ba_debug_inner_iterations(self.handle))
 
+    def debug_eval_list(self, items, count_on_device=False):
+        """[n_obs, 8] per-observation K1 record after K0 + K1 over the observation list `items` (NaN rows elsewhere)"""
+        items = np.ascontiguousarray(items, np.int64)
+        out = np.empty((self.problem.n_obs, 8))
+        _capi.check(self.lib.pxr_ba_debug_eval_list(self.handle, _p(items), C.c_int64(len(items)),
+                                                    int(bool(count_on_device)), _p(out)))
+        return out
+
+    def debug_inner_rounds(self, enable_timing=-1, capacity=64):
+        """rounds of the most recent batched inner iterations: [n, 2] (active observations, active points) per round and
+        the per-round device ms (-1 where round timing was off); enable_timing >= 0 switches round timing for later calls"""
+        counts = np.zeros((capacity, 2), np.uint64); ms = np.zeros(capacity); n = C.c_int()
+        _capi.check(self.lib.pxr_ba_debug_inner_rounds(self.handle, int(enable_timing), int(capacity), _p(counts), _p(ms),
+                                                       C.byref(n)))
+        k = min(n.value, capacity)
+        return counts[:k], ms[:k]
+
     def solve(self, capacity=512):
         s = _capi.make_summary(capacity)
         _capi.check(self.lib.pxr_ba_solve(self.handle, C.byref(s)))
