@@ -274,6 +274,23 @@ int pxr_ba_destroy(pxr_ba* ba);
 int pxr_ba_run(pxr_ctx* ctx, const pxr_ba_desc* desc, const pxr_interp_config* interp,
                const pxr_solver_options* opt, pxr_summary* summary);
 
+/* ---- geometric (reprojection-error) BA -------------------------------------
+ * replaces _bundle_adjustment.GeometricBundleOptimizer (bundle_adjustment/bindings.cc:155-162,
+ * geometric_bundle_optimizer.h:36-83): residual r = WorldToImage(X) - point2D.XY() in image pixels
+ * (colmap::BundleAdjustmentCostFunction through residuals/src/geometric.h:16-41).  The desc carries the geometry, the
+ * constancy masks and the observation lists; its patch fields are unused and must be empty: channels 0, patches,
+ * patch_block_ptrs (n_patch_blocks 0) and refs NULL; corner, scale and obs_patch may be NULL and are ignored.
+ * obs_xy [n_obs][2] is every observation's keypoint (point2D.XY()); a NULL or non-finite entry is
+ * PXR_ERR_INVALID_ARGUMENT.  The handle works with every pxr_ba_* call that takes a pxr_ba; on it pxr_ba_evaluate returns gtr = r,
+ * gtg = (1, 0, 1) and residuals [n_obs][2], pxr_ba_evaluate_jacobians returns grad = the 2x2 identity, and a summary's
+ * num_residuals is 2 n_obs.  The arguments are checked before the context: with ctx == NULL the calls report
+ * PXR_ERR_NO_DEVICE when there is no CUDA device. */
+int pxr_ba_create_geometric(pxr_ctx* ctx, const pxr_ba_desc* desc, const double* obs_xy,
+                            const pxr_solver_options* opt, pxr_ba** out);
+/* one-shot = GeometricBundleOptimizer.run: upload, solve, write back into the desc arrays */
+int pxr_ba_run_geometric(pxr_ctx* ctx, const pxr_ba_desc* desc, const double* obs_xy,
+                         const pxr_solver_options* opt, pxr_summary* summary);
+
 /* Device memory pxr_ba_create / pxr_ba_run will take for this problem, in bytes (host computation, no device needed) —
  * the counterpart of the RAM estimate the reference logs before it solves (bundle_optimizer.h:200-208,
  * util/src/memory.h:45-69).  patch_bytes: the patch slab (0 when it is already resident); state_bytes: per-observation

@@ -66,7 +66,8 @@ int dtype_id(const py::array& a) {
   throw py::value_error("patches must be float16, float32 or float64");
 }
 
-pxr_ba_desc ba_desc(Fields& f) {
+// the geometry and observation lists of a problem dict (every pxr_ba_desc field but the patch ones)
+pxr_ba_desc ba_geometry(Fields& f) {
   pxr_ba_desc d;
   std::memset(&d, 0, sizeof(d));
   d.n_cameras = (int32_t)f.len("cam_model");
@@ -85,6 +86,11 @@ pxr_ba_desc ba_desc(Fields& f) {
   d.n_obs = f.len("obs_img");
   d.obs_img = f.arr<int32_t>("obs_img");
   d.obs_pt = f.arr<int64_t>("obs_pt");
+  return d;
+}
+
+pxr_ba_desc ba_desc(Fields& f) {
+  pxr_ba_desc d = ba_geometry(f);
   d.obs_patch = f.arr<int64_t>("obs_patch", false);
   py::array patches = py::array::ensure(f.d["patches"]);
   if (!patches || patches.ndim() != 4 || !(patches.flags() & py::array::c_style))
@@ -294,6 +300,21 @@ PYBIND11_MODULE(_pxr_pybind, m) {
     check(rc);
     return summary_dict(s, its);
   }, "ctx"_a, "problem"_a, "interpolation"_a = py::dict(), "options"_a = py::dict());
+  // geometric BA (GeometricBundleOptimizer.run): the problem dict holds the geometry and `obs_xy` [n_obs, 2], no patches
+  m.def("ba_run_geometric", [](Context& ctx, py::dict problem, py::dict options) {
+    Fields f{problem, {}};
+    pxr_ba_desc d = ba_geometry(f);
+    const double* obs_xy = f.arr<double>("obs_xy");
+    if (f.len("obs_xy") != d.n_obs) throw py::value_error("obs_xy must hold one keypoint per observation");
+    pxr_solver_options so; pxr_default_ba_options(&so); apply_options(so, options);
+    std::vector<pxr_iteration_summary> its(512);
+    pxr_summary s; std::memset(&s, 0, sizeof(s));
+    s.iterations = its.data(); s.iterations_capacity = (int32_t)its.size();
+    int rc;
+    { py::gil_scoped_release nogil; rc = pxr_ba_run_geometric(ctx.h, &d, obs_xy, &so, &s); }
+    check(rc);
+    return summary_dict(s, its);
+  }, "ctx"_a, "problem"_a, "options"_a = py::dict());
   m.def("refs_compute", [](Context& ctx, py::dict problem, py::dict interpolation, int loss_type, double loss_scale, int iters) {
     Fields f{problem, {}};
     pxr_ba_desc d = ba_desc(f);

@@ -119,9 +119,38 @@ static int check_desc(const pxr_ba_desc* d) {
   return PXR_OK;
 }
 
-int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so, bool for_solve) {
+// A geometric desc: the same geometry and observation lists, no patch slab (channels 0, patches / patch blocks / refs
+// NULL; corner, scale and obs_patch are ignored) and one finite observed keypoint per observation.  Host only.
+static int check_desc_geometric(const pxr_ba_desc* d, const double* obs_xy) {
+  if (!d) return fail(PXR_ERR_INVALID_ARGUMENT, "desc is NULL");
+  if (d->n_cameras <= 0 || d->n_images <= 0 || d->n_points < 0 || d->n_obs < 0)
+    return fail(PXR_ERR_INVALID_ARGUMENT, "empty problem");
+  if (!d->cam_model || !d->cam_params || !d->cam_const_mask || !d->qvec || !d->tvec || !d->img_cam ||
+      !d->pose_const || !d->tvec_const_mask || (d->n_points && (!d->xyz || !d->point_const)) ||
+      (d->n_obs && (!d->obs_img || !d->obs_pt)))
+    return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  if (d->channels != 0 || d->patches || d->n_patch_blocks != 0 || d->refs)
+    return fail(PXR_ERR_INVALID_ARGUMENT, "a geometric problem has no feature patches (channels 0, patches, patch blocks and refs NULL)");
+  if (!obs_xy) return fail(PXR_ERR_INVALID_ARGUMENT, "obs_xy is NULL");
+  for (int c = 0; c < d->n_cameras; ++c)
+    if (cam_num_params(d->cam_model[c]) == 0) return fail(PXR_ERR_UNSUPPORTED, "unsupported camera model id %d", d->cam_model[c]);
+  for (int i = 0; i < d->n_images; ++i)
+    if (d->img_cam[i] < 0 || d->img_cam[i] >= d->n_cameras) return fail(PXR_ERR_INVALID_ARGUMENT, "img_cam out of range");
+  for (int64_t o = 0; o < d->n_obs; ++o) {
+    if (d->obs_img[o] < 0 || d->obs_img[o] >= d->n_images) return fail(PXR_ERR_INVALID_ARGUMENT, "obs_img out of range");
+    if (d->obs_pt[o] < 0 || d->obs_pt[o] >= d->n_points) return fail(PXR_ERR_INVALID_ARGUMENT, "obs_pt out of range");
+    if (o && d->obs_pt[o] < d->obs_pt[o - 1]) return fail(PXR_ERR_INVALID_ARGUMENT, "observations must be sorted by point index");
+    if (!std::isfinite(obs_xy[2 * o]) || !std::isfinite(obs_xy[2 * o + 1]))
+      return fail(PXR_ERR_INVALID_ARGUMENT, "obs_xy[%lld] is not finite", (long long)o);
+  }
+  return PXR_OK;
+}
+
+int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so, bool for_solve,
+               const double* obs_xy) {
   ctx = c;
-  PXR_TRY(check_desc(d));
+  geometric = obs_xy != nullptr;
+  PXR_TRY(geometric ? check_desc_geometric(d, obs_xy) : check_desc(d));
   if (ic) interp = *ic; else pxr_default_interp_config(&interp);
   if (so) opt = *so; else pxr_default_ba_options(&opt);
   if (interp.check_bounds) return fail(PXR_ERR_UNSUPPORTED, "check_bounds=true is not supported on this path");
@@ -136,6 +165,7 @@ int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, co
   n_cameras = d->n_cameras; n_images = d->n_images; n_points = d->n_points; n_obs = d->n_obs;
   C = d->channels; ph = d->ph; pw = d->pw; dtype = d->patch_dtype; ups = d->upsampling_factor;
   n_patches = d->obs_patch ? d->n_patches : std::max(d->n_patches, d->n_obs);
+  if (geometric) { C = 2; ups = 1.0; n_patches = n_obs; }   // two residuals per observation; K0 in the identity patch frame
   has_refs = d->refs != nullptr;
   // the big patch upload goes first, on the context's side stream: the host-side layout / co-visibility work below
   // (and the small synchronous uploads it makes on `s`) overlaps with the DMA; joined when create() returns
@@ -145,7 +175,9 @@ int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, co
   double h2d_patch = 0;
   const size_t esz = dtype == PXR_F16 ? 2 : (dtype == PXR_F32 ? 4 : 8);
   const size_t pbytes = (size_t)n_patches * ph * pw * C * esz;
-  if (d->n_patch_blocks > 0) {
+  if (geometric) {
+    // no patch slab to upload
+  } else if (d->n_patch_blocks > 0) {
     if (!d->patch_block_ptrs || !d->patch_block_counts) return fail(PXR_ERR_INVALID_ARGUMENT, "patch block arrays are NULL");
     int64_t tot = 0;
     for (int b = 0; b < d->n_patch_blocks; ++b) tot += d->patch_block_counts[b];
@@ -203,7 +235,7 @@ int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, co
   auto up = [&](auto& buf, const auto* host, size_t n) -> int { h2d += n * sizeof(*host); return buf.upload(host, n, s); };
   PXR_TRY(up(obs_img, d->obs_img, n_obs));
   PXR_TRY(up(obs_pt, d->obs_pt, n_obs));
-  if (d->obs_patch) PXR_TRY(up(obs_patch, d->obs_patch, n_obs));
+  if (d->obs_patch && !geometric) PXR_TRY(up(obs_patch, d->obs_patch, n_obs));
   PXR_TRY(up(img_cam, d->img_cam, n_images));
   PXR_TRY(up(cam_model, d->cam_model, n_cameras));
   PXR_TRY(up(cam_mask, cmask.data(), n_cameras));
@@ -212,9 +244,13 @@ int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, co
   PXR_TRY(up(intr_off, h_intr_off.data(), n_cameras));
   PXR_TRY(up(point_off, h_point_off.data(), n_points));
   PXR_TRY(up(pt_begin, h_pt_begin.data(), n_points + 1));
-  PXR_TRY(up(corner, d->corner, (size_t)n_patches * 2));
-  PXR_TRY(up(scale, d->scale, (size_t)n_patches * 2));
+  // geometric: identity frame per observation (corner 0, scale 1), so K0's Jacobian record is d(xy)/d(theta) exactly
+  const std::vector<int32_t> geo_corner(geometric ? (size_t)n_obs * 2 : 0, 0);
+  const std::vector<double> geo_scale(geometric ? (size_t)n_obs * 2 : 0, 1.0);
+  PXR_TRY(up(corner, geometric ? geo_corner.data() : d->corner, (size_t)n_patches * 2));
+  PXR_TRY(up(scale, geometric ? geo_scale.data() : d->scale, (size_t)n_patches * 2));
   if (has_refs) PXR_TRY(up(refs, d->refs, (size_t)n_points * C));
+  if (geometric) { PXR_TRY(up(geo_target, obs_xy, (size_t)n_obs * 2)); PXR_TRY(geo_xy.alloc((size_t)n_obs * 2)); }
   for (int k = 0; k < 2; ++k) {
     PXR_TRY(cam[k].upload(d->cam_params, (size_t)n_cameras * kMaxK, s));
     PXR_TRY(q[k].upload(d->qvec, (size_t)n_images * 4, s));
@@ -286,7 +322,8 @@ int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, co
   PXR_TRY(gc.alloc(nc));
   PXR_TRY(Hpp.alloc((size_t)n_points * 9)); PXR_TRY(gp.alloc((size_t)n_points * 3));
   h_obs_img.assign(d->obs_img, d->obs_img + n_obs);
-  use_monolithic_inner = std::getenv("PXR_INNER_MONOLITHIC") != nullptr;
+  // the monolithic kernel interpolates patches itself: a geometric handle always runs the batched rounds
+  use_monolithic_inner = std::getenv("PXR_INNER_MONOLITHIC") != nullptr && !geometric;
   if (for_solve) PXR_TRY(build_schur_pairs());
   if (block_mode) PXR_TRY(block_setup());
   if (for_solve && n_obs > 0 && n_obs < ((int64_t)1 << 31)) {
@@ -460,6 +497,7 @@ int BA::project(int set, bool jac, double* xy_out) {
   a.corner = corner.p; a.scale = scale.p; a.ups = ups;
   a.obs_begin = 0; a.obs_end = n_obs; a.item_index = nullptr;
   a.uv = uv.p; a.xy = xy_out; a.juv = jac ? juv.p : nullptr; a.juv_stride = juv_stride; a.juv_k = K;
+  if (geometric) a.xy = geo_xy.p;     // the geometric residual is formed from the projection itself
   if (n_obs == 0) return PXR_OK;
   StageScope st(this, 2);
   const size_t staged_smem = (size_t)128 * (juv_stride | 1) * sizeof(double);
@@ -468,6 +506,7 @@ int BA::project(int set, bool jac, double* xy_out) {
   else if (jac) PXR_LAUNCH(ctx, ba_project_kernel<true>, (unsigned)cdiv(n_obs, 128), 128, 0, a);
   else PXR_LAUNCH(ctx, ba_project_kernel<false>, (unsigned)cdiv(n_obs, 128), 128, 0, a);
   PXR_CUDA(cudaGetLastError());
+  if (geometric && xy_out) PXR_CUDA(cudaMemcpyAsync(xy_out, geo_xy.p, (size_t)n_obs * 16, cudaMemcpyDeviceToDevice, ctx->stream));
   return PXR_OK;
 }
 
@@ -603,6 +642,10 @@ int BA::fm(int mode, double* residuals_out, double* cost_dev, double* grad_out) 
 
 int BA::fm_k1(int mode, double* residuals_out, double* grad_out, const int64_t* list, int64_t n) {
   if (n <= 0 || n_obs == 0) return PXR_OK;
+  if (geometric) {
+    StageScope st(this, mode ? 1 : 0);
+    return geo_k1(mode, residuals_out, grad_out, list, n);
+  }
   FmEvalArgs a;
   a.uv = uv.p; a.item_patch = obs_patch.p; a.item_ref = obs_pt.p;
   a.patches = d_patches; a.ph = ph; a.pw = pw;
@@ -615,6 +658,21 @@ int BA::fm_k1(int mode, double* residuals_out, double* grad_out, const int64_t* 
   int np = 0;
   StageScope st(this, mode ? 1 : 0);
   return launch_fm_eval(ctx, dtype, C, mode, interp.use_float_simd != 0, a, &np);
+}
+
+// K1 of a geometric handle (pxr_geo.cuh) over all observations or a list; with n_dev the list length is read on the
+// device and n is the upper bound the grid is sized for
+int BA::geo_k1(int mode, double* residuals_out, double* grad_out, const int64_t* list, int64_t n, const unsigned long long* n_dev) {
+  if (n <= 0) return PXR_OK;
+  GeoEvalArgs a;
+  a.xy = geo_xy.p; a.target = geo_target.p;
+  a.begin = 0; a.end = n; a.item_index = list; a.end_dev = n_dev;
+  a.out = obs_out.p; a.residuals = residuals_out; a.grad = grad_out;
+  const unsigned grid = (unsigned)std::min<int64_t>(cdiv(n, 128), (int64_t)ctx->sm_count * 16);
+  if (mode == 1) PXR_LAUNCH(ctx, geo_eval_kernel<1>, grid, 128, 0, a);
+  else PXR_LAUNCH(ctx, geo_eval_kernel<0>, grid, 128, 0, a);
+  PXR_CUDA(cudaGetLastError());
+  return PXR_OK;
 }
 
 int BA::fm_cost(double* cost_dev /* device scalar */) {
@@ -961,8 +1019,9 @@ int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long l
   pa.cam_params = cam[set].p; pa.qvec = q[set].p; pa.tvec = t[set].p; pa.xyz = X[set].p;
   pa.corner = corner.p; pa.scale = scale.p; pa.ups = ups;
   pa.obs_begin = 0; pa.obs_end = n; pa.item_index = list; pa.n_dev = n_dev;
-  pa.uv = uv.p; pa.xy = nullptr; pa.juv = juv.p; pa.juv_stride = juv_stride; pa.juv_k = K;
+  pa.uv = uv.p; pa.xy = geometric ? geo_xy.p : nullptr; pa.juv = juv.p; pa.juv_stride = juv_stride; pa.juv_k = K;
   PXR_LAUNCH(ctx, ba_project_kernel<true>, (unsigned)std::min<int64_t>(cdiv(n, 128), (int64_t)ctx->sm_count * 16), 128, 0, pa);
+  if (geometric) return geo_k1(1, nullptr, nullptr, list, n, n_dev);   // no patches, so nothing for window residency to settle
   FmEvalArgs a;
   a.uv = uv.p; a.item_patch = obs_patch.p; a.item_ref = obs_pt.p;
   a.patches = d_patches; a.ph = ph; a.pw = pw;
@@ -1570,6 +1629,49 @@ int pxr_ba_run(pxr_ctx* ctx, const pxr_ba_desc* desc, const pxr_interp_config* i
   int rc = b->solve(summary);
   if (rc == PXR_OK) rc = b->read_params(desc->cam_params, desc->qvec, desc->tvec, desc->xyz);
   pxr_ba_destroy(h);      // inside the timed call: what the caller waits for
+  if (summary) {
+    summary->d2h_bytes = ((double)desc->n_cameras * kMaxK + desc->n_images * 7.0 + desc->n_points * 3.0) * 8.0;
+    summary->total_time_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  }
+  return rc;
+}
+
+// Geometric BA (GeometricBundleOptimizer): the arguments are checked on the host first, so a bad problem is reported
+// as such on any machine; a NULL context then means there is no device to run on.
+static int geometric_args(pxr_ctx* ctx, const pxr_ba_desc* desc, const double* obs_xy) {
+  PXR_TRY(check_desc_geometric(desc, obs_xy));
+  if (ctx) return PXR_OK;
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
+    cudaGetLastError();
+    return fail(PXR_ERR_NO_DEVICE, "no CUDA device available; libpxr has no CPU fallback");
+  }
+  return fail(PXR_ERR_INVALID_ARGUMENT, "ctx is NULL");
+}
+
+int pxr_ba_create_geometric(pxr_ctx* ctx, const pxr_ba_desc* desc, const double* obs_xy, const pxr_solver_options* opt,
+                            pxr_ba** out) {
+  if (!out) return fail(PXR_ERR_INVALID_ARGUMENT, "out is NULL");
+  PXR_TRY(geometric_args(ctx, desc, obs_xy));
+  BA* b = new BA();
+  const int rc = b->create(ctx, desc, nullptr, opt, true, obs_xy);
+  if (rc != PXR_OK) { delete b; return rc; }
+  *out = reinterpret_cast<pxr_ba*>(b);
+  return PXR_OK;
+}
+
+int pxr_ba_run_geometric(pxr_ctx* ctx, const pxr_ba_desc* desc, const double* obs_xy, const pxr_solver_options* opt,
+                         pxr_summary* summary) {
+  const auto t0 = std::chrono::steady_clock::now();
+  PXR_TRY(geometric_args(ctx, desc, obs_xy));
+  BA* b = new BA();
+  {
+    const int rc0 = b->create(ctx, desc, nullptr, opt, true, obs_xy);
+    if (rc0 != PXR_OK) { delete b; return rc0; }
+  }
+  int rc = b->solve(summary);
+  if (rc == PXR_OK) rc = b->read_params(desc->cam_params, desc->qvec, desc->tvec, desc->xyz);
+  pxr_ba_destroy(reinterpret_cast<pxr_ba*>(b));
   if (summary) {
     summary->d2h_bytes = ((double)desc->n_cameras * kMaxK + desc->n_images * 7.0 + desc->n_points * 3.0) * 8.0;
     summary->total_time_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();

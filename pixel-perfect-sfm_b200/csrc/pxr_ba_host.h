@@ -14,6 +14,7 @@
 #include "pxr_chol.cuh"
 #include "pxr_fm_eval.cuh"
 #include "pxr_fm_small.cuh"
+#include "pxr_geo.cuh"
 #include "pxr_inner.cuh"
 #include "pxr_internal.h"
 #include "pxr_pcg.cuh"
@@ -83,6 +84,10 @@ struct BA {
   int nc = 0, dcmax = 0, juv_stride = 0, img_dc_max = 0;
   double ups = 1.0;
   bool has_refs = false;
+  // geometric (reprojection-error) handle (pxr_ba_create_geometric): no patch slab, K0 in the identity patch frame
+  // writes the projection to geo_xy, K1 is geo_eval_kernel against the observed keypoints geo_target; C = 2
+  bool geometric = false;
+  DevBuf<double> geo_target, geo_xy;
   double h2d_bytes = 0;
   // host layout
   std::vector<int32_t> h_pose_off, h_intr_off;
@@ -192,7 +197,11 @@ struct BA {
   int build_schur_pairs();
   SchurPairs schur_pairs();
 
-  int create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so, bool for_solve);
+  // obs_xy != nullptr: a geometric handle (the desc carries no patches)
+  int create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so, bool for_solve,
+             const double* obs_xy = nullptr);
+  int geo_k1(int mode, double* residuals_out, double* grad_out, const int64_t* list, int64_t n,
+             const unsigned long long* n_dev = nullptr);
   // ---- window residency of the patch slab (pxr_resident.cuh): only in the one-shot pxr_ba_run (the host source must
   // outlive the solve), mapped pinned host source, C >= 8.  A repeated pass is local to the rank, so it composes with the
   // multi-GPU block mode (it only adds a host look at the violation counter after each evaluation).

@@ -295,8 +295,11 @@ def build_problem(reconstruction, feature_view, setup, options, references=None,
         bounds = np.searchsorted(o_img[srt], image_ids)
         bounds = np.append(bounds, len(srt))
         ir._by_image = {int(i): srt[bounds[k]:bounds[k + 1]] for k, i in enumerate(image_ids)}
-    blocks, corners, scales, obs_patch, offsets = _patch_plan(ir, feature_view)
-    ir.slab_offsets = offsets
+    if feature_view is None:       # geometric BA: the observed keypoints instead of feature patches
+        obs_xy = _observed_keypoints(rec, A, o_img, o_p2d)
+    else:
+        blocks, corners, scales, obs_patch, offsets = _patch_plan(ir, feature_view)
+        ir.slab_offsets = offsets
     # parameters of the blocks, in index order
     if isinstance(getattr(rec, "xyz", None), np.ndarray) and hasattr(rec, "point3D_id"):
         rows_i = np.searchsorted(rec.image_id, image_ids); rows_p = np.searchsorted(rec.point3D_id, point_ids)
@@ -311,6 +314,12 @@ def build_problem(reconstruction, feature_view, setup, options, references=None,
         xyz = np.array([rec.points3D[q].xyz for q in ir.point_ids], np.float64).reshape(-1, 3)
         cam_params = [np.asarray(rec.cameras[c].params, np.float64) for c in ir.camera_ids]
         cam_model = np.array([int(rec.cameras[c].model_id) for c in ir.camera_ids], np.int32)
+    if feature_view is None:
+        prob = _capi.BAProblem(cam_model=cam_model, cam_params=cam_params, cam_const_mask=cam_mask, qvec=qvec, tvec=tvec,
+                               img_cam=img_cam, pose_const=pose_const, tvec_const_mask=tmask, xyz=xyz,
+                               point_const=point_const, obs_img=obs_img, obs_pt=obs_pt, patches=None, corner=None,
+                               scale=None, obs_xy=obs_xy)
+        return prob, ir
     refs = None
     if references is not None:
         C_ = feature_view.channels
@@ -328,6 +337,22 @@ def build_problem(reconstruction, feature_view, setup, options, references=None,
                            obs_img=obs_img, obs_pt=obs_pt, patches=None, corner=corners, scale=scales, refs=refs,
                            obs_patch=obs_patch, patch_blocks=blocks)
     return prob, ir
+
+
+def _observed_keypoints(rec, A, obs_image_id, obs_point2D_idx):
+    """[n_obs, 2] point2D.XY() of every observation: what GeometricBundleOptimizer::AddResiduals hands the cost functor
+    (geometric_bundle_optimizer.h:56-73).  An array-backed reconstruction provides them as `p2d_xy` [n_points2D, 2] in
+    the order of its `p2d_begin`."""
+    p2d_xy = getattr(rec, "p2d_xy", None)
+    if p2d_xy is not None:
+        rows = np.searchsorted(A["image_id"], obs_image_id)
+        return np.ascontiguousarray(np.asarray(p2d_xy, np.float64)[A["p2d_begin"][rows] + obs_point2D_idx])
+    if not hasattr(rec, "images") or not hasattr(rec, "points3D"):
+        raise ValueError("geometric bundle adjustment needs the keypoints: an array-backed reconstruction must carry p2d_xy")
+    out = np.empty((len(obs_image_id), 2))
+    for k, (i, j) in enumerate(zip(obs_image_id.tolist(), obs_point2D_idx.tolist())):
+        out[k] = rec.images[i].points2D[j].xy
+    return out
 
 
 class _LazyObs:
@@ -672,6 +697,36 @@ class FeatureReferenceBundleOptimizer:
 
     def summary(self):
         return self._summary
+
+
+class GeometricBundleOptimizer(FeatureReferenceBundleOptimizer):
+    """_bundle_adjustment.GeometricBundleOptimizer(options, setup) (bindings.cc:155-162; geometric_bundle_optimizer.h:
+    11-83): classic bundle adjustment of the reprojection error r = WorldToImage(X) - point2D.XY() in image pixels
+    (colmap::BundleAdjustmentCostFunction).  `run(reconstruction)` = `set_up(reconstruction)` + `solve_problem()`;
+    `summary()`, `problem`, `reset()` as for the featuremetric optimizer.  The problem is built by the same rules; images
+    outside the setup keep their pose constant (ParameterizeImages), which is the geometric functor's constant-pose
+    case (geometric_bundle_optimizer.h:43-45)."""
+    _banner = "Start geometric bundle adjustment."
+
+    def __init__(self, options, setup):
+        super().__init__(options, setup, InterpolationConfig())
+
+    def set_up(self, reconstruction, loss_function=None):
+        """`loss_function`: an optional {"name", "params"} dict used instead of options.loss"""
+        if reconstruction is None:
+            raise ValueError("reconstruction cannot be NULL.")
+        if self._used:
+            raise ValueError("Cannot use the same BundleOptimizer multiple times")
+        self._used = True
+        if loss_function is not None:
+            self.options.loss = dict(loss_function)
+        self._prob, self._ir = build_problem(reconstruction, None, self.setup, self.options)
+        self._reconstruction = reconstruction
+        return True
+
+    def run(self, reconstruction):   # noqa: D102
+        self.set_up(reconstruction)
+        return self.solve_problem()
 
 
 def _loss_id_scale(loss):

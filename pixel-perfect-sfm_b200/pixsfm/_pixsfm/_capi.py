@@ -209,7 +209,9 @@ class BAProblem:
     def __init__(self, cam_model, cam_params, cam_const_mask, qvec, tvec, img_cam, pose_const,
                  tvec_const_mask, xyz, point_const, obs_img, obs_pt, patches, corner, scale,
                  refs=None, obs_patch=None, upsampling_factor=1.0, patches_on_device=False,
-                 patch_shape=None, patch_dtype=None, patch_blocks=None):
+                 patch_shape=None, patch_dtype=None, patch_blocks=None, obs_xy=None):
+        """obs_xy [n_obs, 2]: the observed keypoints of a geometric (reprojection-error) problem; it then has no
+        patches (patches, corner, scale, refs and obs_patch are not used) and two residuals per observation"""
         self.cam_model = _as(cam_model, np.int32)
         nc = len(self.cam_model)
         cp = np.zeros((nc, PXR_MAX_CAM_PARAMS), np.float64)
@@ -236,7 +238,16 @@ class BAProblem:
         self.obs_patch = _as(obs_patch, np.int64)
         self.patches_on_device = bool(patches_on_device)
         self.patch_blocks = None
-        if patch_blocks is not None:
+        self.obs_xy = None
+        if obs_xy is not None:
+            self.obs_xy = _as(obs_xy, np.float64, (-1, 2))
+            if len(self.obs_xy) != len(self.obs_pt):
+                raise ValueError("obs_xy must hold one keypoint per observation")
+            self.obs_patch = None
+            self.patches = None
+            self._patches_ptr = None
+            self.n_patches, self.ph, self.pw, self.channels, self.patch_dtype = 0, 0, 0, 0, 0
+        elif patch_blocks is not None:
             # list of C-contiguous [n_i, H, W, C] arrays (one per FeatureMap), uploaded without concatenation
             blocks = [b for b in patch_blocks]
             for b in blocks:
@@ -272,6 +283,11 @@ class BAProblem:
     @property
     def n_obs(self):
         return len(self.obs_pt)
+
+    @property
+    def residuals_per_obs(self):
+        """2 for a geometric problem, the channel count otherwise"""
+        return 2 if self.obs_xy is not None else self.channels
 
     @property
     def patch_np_dtype(self):

@@ -11,7 +11,8 @@ def _p(a):
 
 
 class BAHandle:
-    """pxr_ba: a BA problem resident on the device (== FeatureReferenceBundleOptimizer.set_up)."""
+    """pxr_ba: a BA problem resident on the device (== FeatureReferenceBundleOptimizer.set_up; a problem with obs_xy
+    is a geometric one, == GeometricBundleOptimizer.set_up)."""
 
     def __init__(self, problem, interp=None, options=None, ctx=None):
         self.ctx = ctx or _capi.default_context()
@@ -21,8 +22,12 @@ class BAHandle:
         self.options = options or _capi.default_ba_options()
         self._desc = problem.desc()
         self.handle = C.c_void_p()
-        _capi.check(self.lib.pxr_ba_create(self.ctx.handle, C.byref(self._desc), C.byref(self.interp),
-                                           C.byref(self.options), C.byref(self.handle)))
+        if problem.obs_xy is not None:      # geometric problem: pxr_ba_create_geometric (the interpolation is not used)
+            _capi.check(self.lib.pxr_ba_create_geometric(self.ctx.handle, C.byref(self._desc), _p(problem.obs_xy),
+                                                         C.byref(self.options), C.byref(self.handle)))
+        else:
+            _capi.check(self.lib.pxr_ba_create(self.ctx.handle, C.byref(self._desc), C.byref(self.interp),
+                                               C.byref(self.options), C.byref(self.handle)))
 
     def close(self):
         if self.handle:
@@ -38,7 +43,7 @@ class BAHandle:
     def evaluate(self, residuals=False):
         n = self.problem.n_obs
         out = dict(sq_norm=np.zeros(n), gtr=np.zeros((n, 2)), gtg=np.zeros((n, 3)), xy=np.zeros((n, 2)))
-        res = np.zeros((n, self.problem.channels)) if residuals else None
+        res = np.zeros((n, self.problem.residuals_per_obs)) if residuals else None
         cost = C.c_double()
         _capi.check(self.lib.pxr_ba_evaluate(self.handle, _p(out["sq_norm"]), _p(out["gtr"]), _p(out["gtg"]),
                                              _p(out["xy"]), _p(res), C.byref(cost)))
@@ -50,7 +55,7 @@ class BAHandle:
     def evaluate_jacobians(self):
         """residuals [n,C], grad [n,2,C] (d r/d u, d r/d v), juv [n,2,9+K] (d(u,v)/d(rot3|t3|X3|cam K)), xy [n,2]:
         pxr_ba_evaluate_jacobians, the factored form of every block's ceres-style Jacobian (J = grad^T-rows x juv)"""
-        n, Cc = self.problem.n_obs, self.problem.channels
+        n, Cc = self.problem.n_obs, self.problem.residuals_per_obs
         kmax = int(np.asarray(self.problem.cam_params).shape[1])
         res, grad, xy = np.zeros((n, Cc)), np.zeros((n, 2, Cc)), np.zeros((n, 2))
         juv = np.zeros((n, 2, 9 + kmax)); w = C.c_int32()
@@ -124,13 +129,17 @@ class BAHandle:
 
 
 def ba_run(problem, interp=None, options=None, ctx=None, capacity=512):
-    """pxr_ba_run: upload, solve, write the refined parameters back into `problem` (in place)."""
+    """pxr_ba_run (pxr_ba_run_geometric for a problem with obs_xy): upload, solve, write the refined parameters back
+    into `problem` (in place)."""
     ctx = ctx or _capi.default_context()
     interp = interp or _capi.default_interp()
     options = options or _capi.default_ba_options()
     d = problem.desc()
     s = _capi.make_summary(capacity)
-    _capi.check(ctx.lib.pxr_ba_run(ctx.handle, C.byref(d), C.byref(interp), C.byref(options), C.byref(s)))
+    if problem.obs_xy is not None:          # geometric problem: pxr_ba_run_geometric
+        _capi.check(ctx.lib.pxr_ba_run_geometric(ctx.handle, C.byref(d), _p(problem.obs_xy), C.byref(options), C.byref(s)))
+    else:
+        _capi.check(ctx.lib.pxr_ba_run(ctx.handle, C.byref(d), C.byref(interp), C.byref(options), C.byref(s)))
     return _capi.summary_to_dict(s)
 
 

@@ -143,8 +143,6 @@ class _GeometricFunctor(_FunctorBase):
         self.tvec = None if tvec is None else np.array(tvec, np.float64).reshape(3)
         self._nres = 2
         self._blocks = [3, self.k] if self.const_pose else [4, 3, 3, self.k]
-        # K0 needs a patch to express (u,v): an identity frame (corner 0, scale 1) makes (u,v) = xy - 0.5
-        self._patch = np.zeros((1, 4, 4, 1), np.float32)
 
     def evaluate(self, *blocks):
         if len(blocks) != len(self._blocks):
@@ -154,17 +152,18 @@ class _GeometricFunctor(_FunctorBase):
             X, cam = (np.asarray(b, np.float64).reshape(-1) for b in blocks)
         else:
             q, t, X, cam = (np.asarray(b, np.float64).reshape(-1) for b in blocks)
+        # a one-observation geometric problem: the residual comes from the geometric evaluation kernel, P = d(xy)/d(theta)
+        # from K0 (G is the identity)
         prob = _capi.BAProblem(cam_model=[self.model], cam_params=[cam], cam_const_mask=[0], qvec=[q], tvec=[t], img_cam=[0],
                                pose_const=[0], tvec_const_mask=[0], xyz=[X], point_const=[0], obs_img=[0], obs_pt=[0],
-                               patches=self._patch, corner=[[0, 0]], scale=[[1.0, 1.0]], refs=None)
-        ic = _capi.default_interp(False, False)
-        h = _engine.BAHandle(prob, ic, _capi.default_ba_options(use_inner_iterations=0))
+                               patches=None, corner=None, scale=None, obs_xy=self.point2D[None])
+        h = _engine.BAHandle(prob, options=_capi.default_ba_options(use_inner_iterations=0))
         try:
             out = h.evaluate_jacobians()
         finally:
             h.close()
         P = out["juv"][0]
-        r = out["xy"][0] - self.point2D
+        r = out["residuals"][0]
         J_X, J_cam = P[:, 6:9].copy(), P[:, 9:9 + self.k].copy()
         if self.const_pose:
             return r, [J_X, J_cam]

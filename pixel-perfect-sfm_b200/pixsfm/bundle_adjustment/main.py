@@ -75,3 +75,20 @@ class CostMapBundleAdjuster(BundleAdjuster, strategy="costmaps"):
         optimizer = ba.CostMapBundleOptimizer(self._optimizer_options(), setup, dict(interpolation, l2_normalize=False))
         optimizer.run(reconstruction, features.FeatureView(costmap_fset, reconstruction))
         return {"costmaps": costmap_fset, "references": references, "summary": optimizer.summary()}
+
+
+class GeometricBundleAdjuster(BundleAdjuster, strategy="geometric"):
+    """classic bundle adjustment of the reprojection error between a 3D point's projection and its keypoint
+    (main.py:289-313), e.g. as the baseline next to featuremetric BA or before / after it.  Needs no features."""
+
+    def refine(self, reconstruction, *args, problem_setup=None):
+        """`*args` takes the feature set `refine_multilevel` passes (unused) and, after it, a positional problem
+        setup.  The reference drops that positional setup and falls back to the default one; here it is honoured, so
+        `refine_multilevel(rec, fm, setup)` adjusts the same images as `refine(rec, problem_setup=setup)`.  One solve
+        per call, so `refine_multilevel` runs one per feature level, as the reference does."""
+        if problem_setup is None and len(args) > 1:
+            problem_setup = args[1]
+        setup = problem_setup if problem_setup is not None else default_problem_setup(reconstruction)
+        optimizer = ba.GeometricBundleOptimizer(self._optimizer_options(), setup)
+        optimizer.run(reconstruction)
+        return {"summary": optimizer.summary()}
