@@ -334,6 +334,12 @@ int pxr_ba_debug_inner_iterations(pxr_ba* ba);
  * observation, NaN elsewhere.  count_on_device = 1 passes n (at most n_obs) through device memory, grids sized for
  * all observations. */
 int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count_on_device, double* out);
+/* Half-warps of the K1 launch (fm_eval_kernel) over n_items items of a (dtype, channels) patch slab, as the library
+ * sizes it on this context's device (tests); 0 for channels < 8, which run one thread per item. */
+int pxr_fm_k1_half_warps(pxr_ctx* ctx, int dtype, int channels, int64_t n_items, int64_t* half_warps);
+/* K0 + K1 in `mode` (0 cost only, 1 Jacobian) over all observations at the current parameters (tests, K1
+ * measurements).  out [n_obs][8]: every observation's record; mode 0 writes s only and leaves the rest NaN. */
+int pxr_ba_debug_eval_records(pxr_ba* ba, int mode, double* out);
 /* The rounds of the most recent batched inner iterations (profiling).  *n_rounds = rounds run; for the first
  * min(*n_rounds, capacity) of them counts[2r] = active observations, counts[2r+1] = active points, and ms[r] = the
  * round's stream time (events around its launches, device idle time waiting for the host included) when round timing
@@ -344,7 +350,8 @@ int pxr_ba_debug_inner_rounds(pxr_ba* ba, int enable_timing, int capacity, unsig
 /* Timing hooks for bench.py: run `iters` LM iterations' worth of the named stage on the
  * resident problem and return the average device time per launch in ms (CUDA events on the
  * library stream).  stage: 0 residual/Jacobian kernel (K1), 1 cost-only kernel, 2 projection+K1+block build,
- * 3 projection kernel (K0), 4 block build, 5 inner-iteration kernel */
+ * 3 projection kernel (K0), 4 block build, 5 inner-iteration kernel, 6 K1 (Jacobian) over a list of every second
+ * observation */
 int pxr_ba_time_stage(pxr_ba* ba, int stage, int iters, double* ms_per_launch);
 /* Device-side synthetic scene generator used by bench.py (data: synthetic). Fills a patch slab
  * on the device from per-patch smooth fields; see DESIGN.md §bench. */

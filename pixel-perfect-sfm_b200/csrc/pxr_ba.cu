@@ -21,6 +21,17 @@
 namespace pxr {
 
 // -------------------------------------------------------------------------------- fm_eval dispatch
+// K1 CTAs for n items: enough for one item per half-warp, up to what is resident; the kernel spreads the items evenly
+// over the half-warps it gets
+template <typename T, int C>
+static int64_t fm_grid(const pxr_ctx* ctx, int64_t n) {
+  typedef FmCfg<T, C> Cfg;
+  int64_t grid = cdiv(n, 2 * Cfg::kWarps);
+  const int64_t resident = (int64_t)ctx->sm_count * std::max(1, (int)(200 * 1024 / Cfg::kSmem));
+  if (grid > resident) grid = resident;
+  return grid < 1 ? 1 : grid;
+}
+
 template <typename T, int C, int MODE, bool FS>
 static int launch_fm(pxr_ctx* ctx, const FmEvalArgs& a, int* n_partials) {
   typedef FmCfg<T, C> Cfg;
@@ -30,11 +41,7 @@ static int launch_fm(pxr_ctx* ctx, const FmEvalArgs& a, int* n_partials) {
     PXR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem));
     attr_set = true;
   }
-  // enough CTAs for one item per warp, up to what is resident: the kernel spreads the items evenly over the warps it gets
-  int64_t grid = cdiv(a.end - a.begin, Cfg::kWarps);
-  const int64_t resident = (int64_t)ctx->sm_count * std::max(1, (int)(200 * 1024 / Cfg::kSmem));
-  if (grid > resident) grid = resident;
-  if (grid < 1) grid = 1;
+  const int64_t grid = fm_grid<T, C>(ctx, a.end - a.begin);
   *n_partials = (int)(grid * Cfg::kWarps);
   PXR_LAUNCH(ctx, kern, (unsigned)grid, Cfg::kWarps * 32, Cfg::kSmem, a);
   PXR_CUDA(cudaGetLastError());
@@ -68,6 +75,17 @@ int fm_supported(int dtype, int C) {
 }
 
 int fm_max_partials(pxr_ctx* ctx) { return ctx->sm_count * 16 * 64; }
+
+// half-warps of the K1 launch over n items (its grid x warps per CTA x 2); 0 for C < 8 (one thread per item)
+static int64_t fm_half_warps(const pxr_ctx* ctx, int dtype, int C, int64_t n) {
+#define PXR_HW(T, CC) \
+  if (C == CC) return fm_grid<T, CC>(ctx, n) * FmCfg<T, CC>::kWarps * 2;
+  if (dtype == PXR_F16) { PXR_HW(__half, 8) PXR_HW(__half, 16) PXR_HW(__half, 32) PXR_HW(__half, 64) PXR_HW(__half, 128) PXR_HW(__half, 256) }
+  else if (dtype == PXR_F32) { PXR_HW(float, 16) PXR_HW(float, 64) PXR_HW(float, 128) }
+  else if (dtype == PXR_F64) { PXR_HW(double, 16) PXR_HW(double, 128) }
+#undef PXR_HW
+  return 0;
+}
 
 int launch_fm_eval(pxr_ctx* ctx, int dtype, int C, int mode, bool float_simd, const FmEvalArgs& a, int* np) {
 #define PXR_SMALL(T) \
@@ -1820,6 +1838,28 @@ int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count
   return PXR_OK;
 }
 
+int pxr_fm_k1_half_warps(pxr_ctx* ctx, int dtype, int channels, int64_t n_items, int64_t* half_warps) {
+  if (!ctx || !half_warps || n_items < 0 || !fm_supported(dtype, channels)) return fail(PXR_ERR_INVALID_ARGUMENT, "bad arguments");
+  *half_warps = fm_half_warps(ctx, dtype, channels, n_items);
+  return PXR_OK;
+}
+
+// K0 + K1 in `mode` (0 cost only, 1 Jacobian) over all observations at the current parameters (tests, K1 measurements):
+// out [n_obs][8] is every observation's record as the pass leaves it (mode 0 writes s only; the rest stays NaN).
+int pxr_ba_debug_eval_records(pxr_ba* ba, int mode, double* out) {
+  if (!ba || (mode != 0 && mode != 1) || !out) return fail(PXR_ERR_INVALID_ARGUMENT, "bad arguments");
+  BA* b = reinterpret_cast<BA*>(ba);
+  pxr_ctx* ctx = b->ctx;
+  cudaStream_t s = ctx->stream;
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  PXR_CUDA(cudaMemsetAsync(b->obs_out.p, 0xff, (size_t)b->n_obs * 64, s));
+  PXR_TRY(b->project(b->cur, true, nullptr));
+  PXR_TRY(b->fm(mode, nullptr, b->scalars.p + 0));
+  PXR_CUDA(cudaMemcpyAsync(out, b->obs_out.p, (size_t)b->n_obs * 64, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  return PXR_OK;
+}
+
 // The rounds of the most recent batched inner iterations (profiling): for every round r < *n_rounds (at most `capacity`
 // are written) counts[2r] active observations and counts[2r+1] active points, and ms[r] its stream time if round timing
 // was on during that call (else -1): events around the round's launches, so any time the device waits for the host to
@@ -1854,11 +1894,18 @@ int pxr_ba_time_stage(pxr_ba* ba, int stage, int iters, double* ms_per_launch) {
   PXR_CUDA(cudaEventCreate(&e0)); PXR_CUDA(cudaEventCreate(&e1));
   double c;
   PXR_TRY(b->project(b->cur, true, nullptr));  // uv for the current parameters
+  DevBuf<int64_t> half_list;                    // stage 6: every second observation
+  if (stage == 6) {
+    std::vector<int64_t> h((size_t)(b->n_obs / 2));
+    for (size_t i = 0; i < h.size(); ++i) h[i] = 2 * (int64_t)i;
+    if (!h.empty()) PXR_TRY(half_list.upload(h.data(), h.size(), s));
+  }
   PXR_CUDA(cudaStreamSynchronize(s));
   PXR_CUDA(cudaEventRecord(e0, s));
   for (int i = 0; i < iters; ++i) {
     if (stage == 0) PXR_TRY(b->fm(1, nullptr, b->scalars.p));
     else if (stage == 1) PXR_TRY(b->fm(0, nullptr, b->scalars.p));
+    else if (stage == 6) PXR_TRY(b->fm_k1(1, nullptr, nullptr, half_list.p, b->n_obs / 2));
     else if (stage == 3) PXR_TRY(b->project(b->cur, true, nullptr));
     else if (stage == 4) PXR_TRY(b->build());
     else if (stage == 5) PXR_TRY(b->inner_iterations(1 - b->cur));

@@ -4,17 +4,17 @@
 //     pixsfm/base/src/projection.h:60-75) + FeaturePatch::ToPixelCoordinates
 //     (features/src/featurepatch.h:250-255) with analytic d(uv)/d(pose,point,intrinsics)
 //     instead of ceres Jets (residuals/src/feature_reference.h:87-96).
-// K1  fm_eval_kernel    : one warp per observation, lane <-> C/32 channels.  The 4x4xC tap
-//     window of the observation's patch is staged HBM -> shared memory by the TMA bulk-copy
-//     engine (cp.async.bulk + mbarrier complete_tx; SASS UBLKCP) through a per-warp ring of
-//     kStages slots, so every warp keeps kStages*4 KiB of loads in flight while it computes.
+// K1  fm_eval_kernel    : one half-warp per observation, lane <-> 2 groups of C/32 channels.  The 4x4xC
+//     tap window of the observation's patch is staged HBM -> shared memory by the TMA bulk-copy
+//     engine (cp.async.bulk + mbarrier complete_tx; SASS UBLKCP) through a per-half-warp ring of
+//     kFmStages slots, so every half-warp keeps kFmStages*4 KiB of loads in flight while it computes.
 //     Border semantics = per-tap clamp (base/src/grid2d.h:29-35): in-range columns are copied
 //     as 4 x (4 taps) contiguous rows, clamped windows fall back to 16 per-tap copies.
 //     Bicubic: horizontal pass in the input's SIMD precision (fp32 for f16/f32), vertical pass in
 //     fp64, same op order as the reference (base/src/interpolation.h:177-218); L2 normalisation
 //     with its chain rule (interpolation.h:648-666); residual r = f - ref
 //     (feature_reference.h:132-134).  The C-channel contraction collapses to
-//     ||r||^2, G^T r (2) and G^T G (3 uniques) by warp shuffles — the per-observation Jacobian is
+//     ||r||^2, G^T r (2) and G^T G (3 uniques) by half-warp shuffles — the per-observation Jacobian is
 //     rank 2 (J = G * d(uv)/d(theta)).
 #pragma once
 #include "pxr_device.cuh"
@@ -140,20 +140,26 @@ __device__ __forceinline__ bool window_resident(uint32_t rect, int row, int col,
 }
 
 #ifndef PXR_FM_WARPS
-#define PXR_FM_WARPS 16
+#define PXR_FM_WARPS 16        // most warps per K1 CTA
 #endif
-constexpr int kFmStages = 2;   // TMA ring slots per warp
-struct FmAux {                 // per-item window geometry, one entry per lane of a batch (40 B)
+constexpr int kFmStages = 2;   // TMA ring slots per half-warp
+// shared memory for the ring slots of one CTA: 128 KiB for windows of up to 4 KiB (fp16 128 channels), 192 KiB for
+// larger ones, which would otherwise leave one warp per scheduler
+template <int SLOT> constexpr int fm_ring_bytes() { return SLOT <= 4096 ? 128 * 1024 : 192 * 1024; }
+struct FmAux {                 // per-item window geometry, one entry per item of a half-warp's batch (40 B)
   double xc, xr;
   int64_t item;
   const uint8_t* src;
   int col, row;
 };
-// warps per CTA so that the ring fits in ~128 KiB of shared memory
+// Warps per CTA: as many as the ring fits into fm_ring_bytes (two halves x kFmStages slots per warp), at most
+// PXR_FM_WARPS.  fp16 128 channels: 8 warps, 151 808 B per CTA (the ring, 32 mbarriers, 512 FmAux entries).  Larger rings were
+// slower on the H100 (DESIGN.md §3, K1 in detail); why was not isolated.
 template <typename T, int C> struct FmCfg {
   static constexpr int kSlot = 16 * C * (int)sizeof(T);
-  static constexpr int kWarps = kSlot <= 4096 ? PXR_FM_WARPS : (kSlot <= 8192 ? 8 : (kSlot <= 16384 ? 4 : 2));
-  static constexpr int kSmem = kWarps * kFmStages * kSlot + kWarps * kFmStages * 8 + kWarps * 32 * (int)sizeof(FmAux);
+  static constexpr int kFit = fm_ring_bytes<kSlot>() / (2 * kFmStages * kSlot);
+  static constexpr int kWarps = kFit < 1 ? 1 : (kFit > PXR_FM_WARPS ? PXR_FM_WARPS : kFit);
+  static constexpr int kSmem = kWarps * (2 * kFmStages * kSlot + 2 * kFmStages * 8 + 64 * (int)sizeof(FmAux));
 };
 
 template <typename T> struct HorizT { typedef float type; };
@@ -351,55 +357,181 @@ __device__ __forceinline__ double normalize_and_reduce(bool active, bool l2, con
   return warp_reduce8_transposed(v, lane);
 }
 
+// ---------------------------------------------------------------------------------------------
+// K1 runs one observation per half-warp.  Lane q (0-15) of a half holds the channels lanes q and q + 16 of a
+// warp-per-observation layout would hold: group A at q*CPL and group B at (q+16)*CPL.  Every fp64 sum over the
+// channels is the butterfly of that layout, levels 16, 8, 4, 2, 1: a lane forms each group's partial on its own, the
+// xor-16 level becomes the in-lane sum A + B, and levels 8, 4, 2, 1 stay inside the half.  The records are therefore
+// bit-identical to a warp per observation, and one shuffle serves two observations.
+
+// levels 8, 4, 2, 1 of the butterfly: every lane of the half gets the half's total
+__device__ __forceinline__ double half_sum(double v) {
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Transposed reduction of 8 per-lane doubles over each half-warp (levels 8, 4, 2, 1), 8 double shuffles for both halves.
+// On return lane L holds the half's total of value index ((L>>3)&1)*4 + ((L>>2)&1)*2 + ((L>>1)&1).
+__device__ __forceinline__ double half_reduce8_transposed(const double v[8], int lane) {
+  const bool b3 = lane & 8, b2 = lane & 4, b1 = lane & 2;
+  double a[4], b[2];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const double keep = b3 ? v[4 + j] : v[j];
+    const double send = b3 ? v[j] : v[4 + j];
+    a[j] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+  }
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const double keep = b2 ? a[2 + j] : a[j];
+    const double send = b2 ? a[j] : a[2 + j];
+    b[j] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+  }
+  const double keep = b1 ? b[1] : b[0];
+  const double send = b1 ? b[0] : b[1];
+  double c = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+  c += __shfl_xor_sync(0xffffffffu, c, 1);
+  return c;
+}
+
+// One channel group's share of the L2 norm, the residual and the rank-2 terms, with the operation order of a lane of
+// the warp-per-observation layout.
+template <int CPL>
+__device__ __forceinline__ double group_sq_norm(bool active, const double f[CPL]) {
+  double n2 = 0.0;
+  if (active) {
+#pragma unroll
+    for (int k = 0; k < CPL; ++k) n2 += f[k] * f[k];
+  }
+  return n2;
+}
+template <int CPL, bool DERIV>
+__device__ __forceinline__ void group_scale(bool active, double ninv, double f[CPL], double fr[CPL], double fc[CPL],
+                                            double& dc, double& dr) {
+  dc = 0.0; dr = 0.0;
+#pragma unroll
+  for (int k = 0; k < CPL; ++k) {
+    f[k] *= ninv;
+    if (DERIV) { fc[k] *= ninv; fr[k] *= ninv; if (active) { dc += f[k] * fc[k]; dr += f[k] * fr[k]; } }
+  }
+}
+template <int CPL>
+__device__ __forceinline__ void group_project(double dc, double dr, const double f[CPL], double fr[CPL], double fc[CPL]) {
+#pragma unroll
+  for (int k = 0; k < CPL; ++k) { fc[k] -= dc * f[k]; fr[k] -= dr * f[k]; }
+}
+template <int CPL, bool DERIV>
+__device__ __forceinline__ void group_terms(bool active, bool has_ref, const double refv[CPL], const double f[CPL],
+                                            const double fr[CPL], const double fc[CPL], double r[CPL], double v[8]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) v[i] = 0.0;
+  if (active) {
+#pragma unroll
+    for (int k = 0; k < CPL; ++k) {
+      r[k] = has_ref ? f[k] - refv[k] : f[k];
+      v[0] += r[k] * r[k];
+      if (DERIV) {
+        v[1] += fc[k] * r[k]; v[2] += fr[k] * r[k];
+        v[3] += fc[k] * fc[k]; v[4] += fc[k] * fr[k]; v[5] += fr[k] * fr[k];
+      }
+    }
+  }
+}
+
+// PixelInterpolator L2 normalisation + residual + rank-2 reduction of the observation of a half-warp (groups A and B).
+// Returns, MODE 0: ||r||^2 in every lane; MODE 1: the transposed totals of half_reduce8_transposed
+// (0:s 1:b_u 2:b_v 3:a_uu 4:a_uv 5:a_vv).
+template <int CPL, bool DERIV>
+__device__ __forceinline__ double normalize_and_reduce_half(bool act_a, bool act_b, bool l2, bool has_ref,
+                                                            const double ref_a[CPL], const double ref_b[CPL],
+                                                            double fa[CPL], double fra[CPL], double fca[CPL], double ra[CPL],
+                                                            double fb[CPL], double frb[CPL], double fcb[CPL], double rb[CPL],
+                                                            int lane) {
+  if (l2) {
+    const double n2a = group_sq_norm<CPL>(act_a, fa), n2b = group_sq_norm<CPL>(act_b, fb);
+    const double ninv = 1.0 / sqrt(half_sum(n2a + n2b));
+    double dca, dra, dcb, drb;
+    group_scale<CPL, DERIV>(act_a, ninv, fa, fra, fca, dca, dra);
+    group_scale<CPL, DERIV>(act_b, ninv, fb, frb, fcb, dcb, drb);
+    if (DERIV) {
+      const double dc = half_sum(dca + dcb), dr = half_sum(dra + drb);
+      group_project<CPL>(dc, dr, fa, fra, fca);
+      group_project<CPL>(dc, dr, fb, frb, fcb);
+    }
+  }
+  double va[8], vb[8];
+  group_terms<CPL, DERIV>(act_a, has_ref, ref_a, fa, fra, fca, ra, va);
+  group_terms<CPL, DERIV>(act_b, has_ref, ref_b, fb, frb, fcb, rb, vb);
+  if (!DERIV) return half_sum(va[0] + vb[0]);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) va[i] += vb[i];
+  return half_reduce8_transposed(va, lane);
+}
+
+// the CPL channels of one group to out[item * C + ch0 ..]
+template <int CPL>
+__device__ __forceinline__ void store_group(double* out, int64_t row, int C, int ch0, const double v[CPL]) {
+#pragma unroll
+  for (int k = 0; k < CPL; ++k) out[row * C + ch0 + k] = v[k];
+}
+
 // MODE 0: cost only (f), MODE 1: value + derivatives
 template <typename T, int C, int MODE, bool FLOAT_SIMD>
 __global__ void __launch_bounds__(FmCfg<T, C>::kWarps * 32, 1) fm_eval_kernel(FmEvalArgs a) {
   constexpr int kFmWarps = FmCfg<T, C>::kWarps;
   constexpr bool DERIV = MODE == 1;
   constexpr int CPL = C >= 32 ? C / 32 : 1;
-  constexpr int ACTIVE = C / CPL;
+  constexpr int ACTIVE = C / CPL;             // channel lanes of the warp-per-observation layout
   constexpr int TAP_BYTES = C * (int)sizeof(T);
   constexpr int SLOT_BYTES = 16 * TAP_BYTES;
   static_assert(TAP_BYTES % 16 == 0, "bulk copies need 16-byte multiples");
   extern __shared__ __align__(128) uint8_t smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  uint8_t* wbase = smem + (size_t)warp * kFmStages * SLOT_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)kFmWarps * kFmStages * SLOT_BYTES) + warp * kFmStages;
-  FmAux* aux = reinterpret_cast<FmAux*>(smem + (size_t)kFmWarps * kFmStages * SLOT_BYTES + kFmWarps * kFmStages * 8) + warp * 32;
-  if (lane == 0) {
+  const int half = lane >> 4, q = lane & 15;
+  const int hw = warp * 2 + half;             // half-warp of the CTA
+  uint8_t* hbase = smem + (size_t)hw * kFmStages * SLOT_BYTES;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)kFmWarps * 2 * kFmStages * SLOT_BYTES) + hw * kFmStages;
+  FmAux* aux = reinterpret_cast<FmAux*>(smem + (size_t)kFmWarps * 2 * kFmStages * SLOT_BYTES + kFmWarps * 2 * kFmStages * 8) + hw * 32;
+  if (q == 0) {
 #pragma unroll
     for (int s = 0; s < kFmStages; ++s) mbar_init(&bars[s], 1);
     mbar_fence_init();
   }
   __syncwarp();
-  const bool active = lane < ACTIVE;
+  const bool act_a = q < ACTIVE, act_b = q + 16 < ACTIVE;
   const int64_t item_end = a.end_dev ? a.begin + (int64_t)*a.end_dev : a.end;
   const int64_t n_items = item_end - a.begin;
-  const int64_t warp_global = (int64_t)blockIdx.x * kFmWarps + warp;
-  const int64_t warps_total = (int64_t)gridDim.x * kFmWarps;
-  // balanced batches: every warp walks at most R = ceil(n / (32 W)) batches of bsz = ceil(n / (W R)) <= 32 consecutive items,
-  // so a short list spreads one or two items over every warp and a long one leaves no partial last wave of 32-item batches
-  const int64_t rounds = n_items > 0 ? (n_items + 32 * warps_total - 1) / (32 * warps_total) : 0;
-  const int bsz = rounds > 0 ? (int)((n_items + warps_total * rounds - 1) / (warps_total * rounds)) : 32;
+  const int64_t halves_total = (int64_t)gridDim.x * kFmWarps * 2;
+  // balanced batches: every half-warp walks at most R = ceil(n / (32 W2)) batches of bsz = ceil(n / (W2 R)) <= 32
+  // consecutive items (W2 half-warps in the launch), so a short list spreads one item over every half-warp and a long one
+  // leaves no partial last wave of 32-item batches.  The halves of a warp take consecutive batches, so half 1 never has
+  // more items than half 0; past its last item a half computes nothing it stores.
+  const int64_t rounds = n_items > 0 ? (n_items + 32 * halves_total - 1) / (32 * halves_total) : 0;
+  const int bsz = rounds > 0 ? (int)((n_items + halves_total * rounds - 1) / (halves_total * rounds)) : 32;
   const int64_t n_batches = rounds > 0 ? (n_items + bsz - 1) / bsz : 0;
   uint32_t phase_bits = 0;
   const int64_t patch_bytes = (int64_t)a.ph * a.pw * TAP_BYTES;
   const bool has_ref = a.refs != nullptr;
 
-  for (int64_t batch = warp_global; batch < n_batches; batch += warps_total) {
-    const int nvalid = (int)min((int64_t)bsz, item_end - (a.begin + batch * bsz));
-    int64_t o = a.begin + batch * bsz + lane;
-    if (a.item_index && lane < nvalid) o = a.item_index[o];
-    // ---- phase 1: per-lane window geometry, published to the warp through shared memory
+  for (int64_t batch0 = ((int64_t)blockIdx.x * kFmWarps + warp) * 2; batch0 < n_batches; batch0 += halves_total) {
+    const int64_t batch = batch0 + half;
+    const int nvalid = batch < n_batches ? (int)min((int64_t)bsz, item_end - (a.begin + batch * bsz)) : 0;
+    const int nwarp = __shfl_sync(0xffffffffu, nvalid, 0);   // half 0's count, the larger one
+    // ---- phase 1: window geometry of items q and q + 16 of the half's batch, published through shared memory
     __syncwarp();
-    int64_t ref_idx = 0;
-    {
+    int64_t ref_idx[2] = {0, 0};
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const int jj = q + 16 * s;
+      int64_t o = a.begin + batch * bsz + jj;
       double u = 0.0, v = 0.0;
-      int64_t pidx = 0, ridx = 0;
-      if (lane < nvalid) {
+      int64_t pidx = 0;
+      if (jj < nvalid) {
+        if (a.item_index) o = a.item_index[o];
         u = a.uv[2 * o]; v = a.uv[2 * o + 1];
         pidx = a.item_patch ? a.item_patch[o] : o;
-        ridx = a.item_ref ? a.item_ref[o] : o;
+        ref_idx[s] = a.item_ref ? a.item_ref[o] : o;
       }
       const double fu = floor(u), fv = floor(v);
       // guard the int conversion (NaN/huge projections clamp to the border like any far-away tap)
@@ -409,82 +541,89 @@ __global__ void __launch_bounds__(FmCfg<T, C>::kWarps * 32, 1) fm_eval_kernel(Fm
       x.row = (int)fmin(fmax(fv, -4.0), (double)a.ph + 4.0);
       x.xc = u - fu; x.xr = v - fv;
       x.src = a.patches + pidx * patch_bytes;
-      aux[lane] = x;
-      ref_idx = ridx;
-      if (a.res_rect && lane < nvalid && !window_resident(a.res_rect[pidx], x.row, x.col, a.ph, a.pw)) {
+      aux[jj] = x;
+      if (a.res_rect && jj < nvalid && !window_resident(a.res_rect[pidx], x.row, x.col, a.ph, a.pw)) {
         const unsigned long long slot = atomicAdd(a.viol_count, 1ull);
         if ((long long)slot < a.viol_capacity) a.viol_list[slot] = o;
       }
     }
     __syncwarp();
 
+    // the 4x4 tap window of item j into slot `slot` of the half's ring (lanes of one half; the other may be idle)
     auto issue = [&](int j, int slot) {
       const int jc = aux[j].col, jr = aux[j].row;
       const uint8_t* src = aux[j].src;
-      uint8_t* dst = wbase + (size_t)slot * SLOT_BYTES;
-      if (lane == 0) mbar_expect_tx(&bars[slot], SLOT_BYTES);
-      __syncwarp();
+      uint8_t* dst = hbase + (size_t)slot * SLOT_BYTES;
+      if (q == 0) mbar_expect_tx(&bars[slot], SLOT_BYTES);
       const bool contiguous = (jc - 1 >= 0) && (jc + 2 <= a.pw - 1);
       if (contiguous) {
-        if (lane < 4) {
-          const int rr = min(max(jr - 1 + lane, 0), a.ph - 1);
-          bulk_g2s(dst + lane * 4 * TAP_BYTES, src + ((int64_t)rr * a.pw + (jc - 1)) * TAP_BYTES, 4 * TAP_BYTES, &bars[slot]);
+        if (q < 4) {
+          const int rr = min(max(jr - 1 + q, 0), a.ph - 1);
+          bulk_g2s(dst + q * 4 * TAP_BYTES, src + ((int64_t)rr * a.pw + (jc - 1)) * TAP_BYTES, 4 * TAP_BYTES, &bars[slot]);
         }
-      } else if (lane < 16) {
-        const int rr = min(max(jr - 1 + (lane >> 2), 0), a.ph - 1);
-        const int cc = min(max(jc - 1 + (lane & 3), 0), a.pw - 1);
-        bulk_g2s(dst + lane * TAP_BYTES, src + ((int64_t)rr * a.pw + cc) * TAP_BYTES, TAP_BYTES, &bars[slot]);
+      } else {
+        const int rr = min(max(jr - 1 + (q >> 2), 0), a.ph - 1);
+        const int cc = min(max(jc - 1 + (q & 3), 0), a.pw - 1);
+        bulk_g2s(dst + q * TAP_BYTES, src + ((int64_t)rr * a.pw + cc) * TAP_BYTES, TAP_BYTES, &bars[slot]);
       }
     };
 
-    // ---- phase 2: software pipeline over the batch
+    // ---- phase 2: software pipeline over the batch, both halves in step
 #pragma unroll
     for (int s = 0; s < kFmStages; ++s)
       if (s < nvalid) issue(s, s);
-    for (int j = 0; j < nvalid; ++j) {
+    __syncwarp();
+    for (int j = 0; j < nwarp; ++j) {
+      const bool valid = j < nvalid;
       const int slot = j % kFmStages;
       const double jxc = aux[j].xc, jxr = aux[j].xr;
-      double refv[CPL];
-      if (has_ref) {
-        const int64_t jref = __shfl_sync(0xffffffffu, (long long)ref_idx, j);
-        const double* rp = a.refs + jref * C + (active ? lane * CPL : 0);
+      const int64_t jref = __shfl_sync(0xffffffffu, (long long)(j < 16 ? ref_idx[0] : ref_idx[1]), (lane & 16) | (j & 15));
+      double ref_a[CPL], ref_b[CPL];
 #pragma unroll
-        for (int k = 0; k < CPL; ++k) refv[k] = __ldg(rp + k);
+      for (int k = 0; k < CPL; ++k) { ref_a[k] = 0.0; ref_b[k] = 0.0; }
+      if (has_ref && valid) {
+        const double* rp = a.refs + jref * C;
+#pragma unroll
+        for (int k = 0; k < CPL; ++k) ref_a[k] = __ldg(rp + (act_a ? q * CPL : 0) + k);
+        if (act_b) {
+#pragma unroll
+          for (int k = 0; k < CPL; ++k) ref_b[k] = __ldg(rp + (q + 16) * CPL + k);
+        }
       }
-      mbar_wait(&bars[slot], (phase_bits >> slot) & 1u);
-      phase_bits ^= (1u << slot);
-      double f[CPL], fr[CPL], fc[CPL], r[CPL], red[6];
+      double fa[CPL], fra[CPL], fca[CPL], ra[CPL], fb[CPL], frb[CPL], fcb[CPL], rb[CPL];
 #pragma unroll
-      for (int k = 0; k < CPL; ++k) { f[k] = 0; fr[k] = 0; fc[k] = 0; r[k] = 0; }
-      if (active) {
-        const SmemWindow<TAP_BYTES> win{wbase + (size_t)slot * SLOT_BYTES};
-        bicubic_window<T, C, CPL, DERIV, FLOAT_SIMD>(win, lane, jxc, jxr, f, fr, fc);
+      for (int k = 0; k < CPL; ++k) { fa[k] = 0; fra[k] = 0; fca[k] = 0; ra[k] = 0; fb[k] = 0; frb[k] = 0; fcb[k] = 0; rb[k] = 0; }
+      if (valid) {
+        mbar_wait(&bars[slot], (phase_bits >> slot) & 1u);
+        phase_bits ^= (1u << slot);
+        const SmemWindow<TAP_BYTES> win{hbase + (size_t)slot * SLOT_BYTES};
+        if (act_a) bicubic_window<T, C, CPL, DERIV, FLOAT_SIMD>(win, q, jxc, jxr, fa, fra, fca);
+        if (act_b) bicubic_window<T, C, CPL, DERIV, FLOAT_SIMD>(win, q + 16, jxc, jxr, fb, frb, fcb);
       }
       __syncwarp();
-      if (j + kFmStages < nvalid) issue(j + kFmStages, slot);  // refill the slot just consumed
-      const double tot = normalize_and_reduce<CPL, DERIV, false>(active, a.l2_normalize != 0, has_ref ? refv : nullptr, f, fr, fc, r, red, lane);
+      if (valid && j + kFmStages < nvalid) issue(j + kFmStages, slot);  // refill the slot just consumed
+      const double tot = normalize_and_reduce_half<CPL, DERIV>(act_a, act_b, a.l2_normalize != 0, has_ref, ref_a, ref_b,
+                                                               fa, fra, fca, ra, fb, frb, fcb, rb, lane);
+      if (!valid) continue;
       const int64_t oj = aux[j].item;
-      if (a.residuals && active) {
-#pragma unroll
-        for (int k = 0; k < CPL; ++k) a.residuals[oj * C + lane * CPL + k] = r[k];
+      if (a.residuals) {
+        if (act_a) store_group<CPL>(a.residuals, oj, C, q * CPL, ra);
+        if (act_b) store_group<CPL>(a.residuals, oj, C, (q + 16) * CPL, rb);
       }
-      if (a.desc && active) {
-#pragma unroll
-        for (int k = 0; k < CPL; ++k) a.desc[oj * C + lane * CPL + k] = f[k];
+      if (a.desc) {
+        if (act_a) store_group<CPL>(a.desc, oj, C, q * CPL, fa);
+        if (act_b) store_group<CPL>(a.desc, oj, C, (q + 16) * CPL, fb);
       }
-      if (DERIV && a.grad && active) {
-#pragma unroll
-        for (int k = 0; k < CPL; ++k) {
-          a.grad[(oj * 2) * C + lane * CPL + k] = fc[k];
-          a.grad[(oj * 2 + 1) * C + lane * CPL + k] = fr[k];
-        }
+      if (DERIV && a.grad) {
+        if (act_a) { store_group<CPL>(a.grad, 2 * oj, C, q * CPL, fca); store_group<CPL>(a.grad, 2 * oj + 1, C, q * CPL, fra); }
+        if (act_b) { store_group<CPL>(a.grad, 2 * oj, C, (q + 16) * CPL, fcb); store_group<CPL>(a.grad, 2 * oj + 1, C, (q + 16) * CPL, frb); }
       }
       if (a.out) {
         if (DERIV) {
-          // lanes 0,4,..,28 hold s, a_vv?...: value index = bit4*4 + bit3*2 + bit2
-          const int idx = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-          if ((lane & 3) == 0 && idx < 6) a.out[oj * 8 + idx] = tot;
-        } else if (lane == 0) {
+          // lanes q = 0, 2, .., 10 of each half hold s, b_u, b_v, a_uu, a_uv, a_vv: value index = bit3*4 + bit2*2 + bit1
+          const int idx = ((q >> 3) & 1) * 4 + ((q >> 2) & 1) * 2 + ((q >> 1) & 1);
+          if ((q & 1) == 0 && idx < 6) a.out[oj * 8 + idx] = tot;
+        } else if (q == 0) {
           a.out[oj * 8] = tot;
         }
       }

@@ -87,6 +87,13 @@ class BAHandle:
                                                     int(bool(count_on_device)), _p(out)))
         return out
 
+    def debug_eval_records(self, mode=1):
+        """[n_obs, 8] per-observation K1 record after K0 + K1 over all observations, mode 0 (cost only: column 0, NaN
+        elsewhere) or 1 (Jacobian)"""
+        out = np.empty((self.problem.n_obs, 8))
+        _capi.check(self.lib.pxr_ba_debug_eval_records(self.handle, int(mode), _p(out)))
+        return out
+
     def debug_inner_rounds(self, enable_timing=-1, capacity=64):
         """rounds of the most recent batched inner iterations: [n, 2] (active observations, active points) per round and
         the per-round device ms (-1 where round timing was off); enable_timing >= 0 switches round timing for later calls"""
@@ -126,6 +133,15 @@ class BAHandle:
         ms = C.c_double()
         _capi.check(self.lib.pxr_ba_time_stage(self.handle, int(stage), int(iters), C.byref(ms)))
         return ms.value
+
+
+def k1_half_warps(dtype, channels, n_items, ctx=None):
+    """pxr_fm_k1_half_warps: half-warps of the K1 launch over n_items items of a (dtype, channels) patch slab"""
+    ctx = ctx or _capi.default_context()
+    hw = C.c_int64()
+    _capi.check(ctx.lib.pxr_fm_k1_half_warps(ctx.handle, _capi.DTYPE_IDS[np.dtype(dtype)], int(channels),
+                                              C.c_int64(int(n_items)), C.byref(hw)))
+    return hw.value
 
 
 def ba_run(problem, interp=None, options=None, ctx=None, capacity=512):
