@@ -334,6 +334,19 @@ int pxr_ba_debug_inner_iterations(pxr_ba* ba);
  * observation, NaN elsewhere.  count_on_device = 1 passes n (at most n_obs) through device memory, grids sized for
  * all observations. */
 int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count_on_device, double* out);
+/* The point-only projection of the inner-iteration rounds next to the full one (tests), at the current parameters:
+ * uv_full [n_obs][2] from the full projection (K0 with Jacobians) over all observations, then uv [n_obs][2] and
+ * jpt [n_obs][6] (d(uv)/dX: row u, then row v) from the point-only projection over list[0..n), NaN elsewhere.
+ * count_on_device as in pxr_ba_debug_eval_list. */
+int pxr_ba_debug_project_point(pxr_ba* ba, const int64_t* list, int64_t n, int count_on_device, double* uv, double* jpt,
+                               double* uv_full);
+/* Batched inner iterations run with capture on (enable = 1) keep each round's lists (tests; the host waits for every
+ * round).  pxr_ba_debug_inner_round_lists then reads round `round` of the most recent call: *n_points / *n_obs its list
+ * lengths, plist [*n_points] its points, list [*n_obs] its observations, active [*n_points] 1 where the round's step
+ * kernel kept the point active.  Any output may be NULL. */
+int pxr_ba_debug_inner_capture(pxr_ba* ba, int enable);
+int pxr_ba_debug_inner_round_lists(pxr_ba* ba, int round, int64_t* plist, int64_t* list, uint8_t* active, int64_t* n_points,
+                                   int64_t* n_obs);
 /* Half-warps of the K1 launch (fm_eval_kernel) over n_items items of a (dtype, channels) patch slab, as the library
  * sizes it on this context's device (tests); 0 for channels < 8, which run one thread per item. */
 int pxr_fm_k1_half_warps(pxr_ctx* ctx, int dtype, int channels, int64_t n_items, int64_t* half_warps);
@@ -347,6 +360,10 @@ int pxr_ba_debug_eval_records(pxr_ba* ba, int mode, double* out);
  * on / off for the calls that follow.  Any output may be NULL. */
 int pxr_ba_debug_inner_rounds(pxr_ba* ba, int enable_timing, int capacity, unsigned long long* counts, double* ms,
                               int* n_rounds);
+/* The same rounds split by launch (profiling), when round timing was on during that call (else -1): ms[3r] from the
+ * round's start to the end of K0 (the projection), ms[3r+1] from there to the end of K1 (fm_eval_kernel), ms[3r+2]
+ * from there to the end of the step kernel.  Stream time, so each part includes the launch gap before its kernel. */
+int pxr_ba_debug_inner_round_split(pxr_ba* ba, int capacity, double* ms, int* n_rounds);
 /* Timing hooks for bench.py: run `iters` LM iterations' worth of the named stage on the
  * resident problem and return the average device time per launch in ms (CUDA events on the
  * library stream).  stage: 0 residual/Jacobian kernel (K1), 1 cost-only kernel, 2 projection+K1+block build,

@@ -1026,20 +1026,45 @@ int BA::apply_step(double* step_norm, double* x_norm) {
   return PXR_OK;
 }
 
-// K0 (with Jacobians) + K1 (Jacobian mode) over an explicit list of observations.  With n_dev the number of entries is
-// read on the device (n is then the upper bound the grids are sized for); settle = false leaves the window-residency
-// check to the caller (inner_rounds checks once per batch of rounds).
-int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev, bool settle) {
-  if (n <= 0) return PXR_OK;
+// ba_project_point_kernel over list[0..n) (or [0..*n_dev), grid sized for n): uv (xy on a geometric handle) and d(uv)/dX
+// to inner_jpt.
+int BA::alloc_inner_jpt() {
+  if (!inner_jpt.p) PXR_TRY(inner_jpt.alloc((size_t)n_obs * 6));
+  return PXR_OK;
+}
+
+int BA::project_point_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev, int64_t grid_bound) {
+  if (!inner_jpt.p) return fail(PXR_ERR_INTERNAL, "the point-only projection ran before its buffer was allocated");
+  if (grid_bound <= 0) return PXR_OK;
   ProjectArgs pa;
   pa.obs_img = obs_img.p; pa.obs_pt = obs_pt.p; pa.obs_patch = obs_patch.p;
   pa.img_cam = img_cam.p; pa.cam_model = cam_model.p;
   pa.cam_params = cam[set].p; pa.qvec = q[set].p; pa.tvec = t[set].p; pa.xyz = X[set].p;
   pa.corner = corner.p; pa.scale = scale.p; pa.ups = ups;
   pa.obs_begin = 0; pa.obs_end = n; pa.item_index = list; pa.n_dev = n_dev;
-  pa.uv = uv.p; pa.xy = geometric ? geo_xy.p : nullptr; pa.juv = juv.p; pa.juv_stride = juv_stride; pa.juv_k = K;
-  PXR_LAUNCH(ctx, ba_project_kernel<true>, (unsigned)std::min<int64_t>(cdiv(n, 128), (int64_t)ctx->sm_count * 16), 128, 0, pa);
-  if (geometric) return geo_k1(1, nullptr, nullptr, list, n, n_dev);   // no patches, so nothing for window residency to settle
+  pa.uv = uv.p; pa.xy = geometric ? geo_xy.p : nullptr; pa.juv = nullptr; pa.juv_stride = juv_stride; pa.juv_k = K;
+  pa.jpt = inner_jpt.p;
+  PXR_LAUNCH(ctx, ba_project_point_kernel, (unsigned)std::min<int64_t>(cdiv(grid_bound, 128), (int64_t)ctx->sm_count * 16), 128,
+             (size_t)128 * (juv_stride | 1) * sizeof(double), pa);
+  return PXR_OK;
+}
+
+// K0 (uv and the point Jacobian only, to inner_jpt) + K1 (Jacobian mode) over an explicit list of observations, what
+// an inner-iteration round evaluates: its step kernel reads d(uv)/dX and nothing else of the Jacobian, and the driver
+// projects afresh after the rounds, so juv is left alone.  With n_dev the number of entries is read on the device (n is
+// then the upper bound K1's grid is sized for, k0_bound, when >= 0, a tighter one for K0's); settle = false leaves the
+// window-residency check to the caller (inner_rounds checks once per batch of rounds).  after_k0 / after_k1, when
+// given, are recorded right after the K0 and K1 launches (round timing).
+int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev, bool settle,
+                  cudaEvent_t after_k0, cudaEvent_t after_k1, int64_t k0_bound) {
+  if (n <= 0) return PXR_OK;
+  PXR_TRY(project_point_list(set, list, n, n_dev, k0_bound >= 0 ? std::min(k0_bound, n) : n));
+  if (after_k0) PXR_CUDA(cudaEventRecord(after_k0, ctx->stream));
+  if (geometric) {   // no patches, so nothing for window residency to settle
+    PXR_TRY(geo_k1(1, nullptr, nullptr, list, n, n_dev));
+    if (after_k1) PXR_CUDA(cudaEventRecord(after_k1, ctx->stream));
+    return PXR_OK;
+  }
   FmEvalArgs a;
   a.uv = uv.p; a.item_patch = obs_patch.p; a.item_ref = obs_pt.p;
   a.patches = d_patches; a.ph = ph; a.pw = pw;
@@ -1051,6 +1076,7 @@ int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long l
   resident_args(a);
   int np = 0;
   PXR_TRY(launch_fm_eval(ctx, dtype, C, 1, interp.use_float_simd != 0, a, &np));
+  if (after_k1) PXR_CUDA(cudaEventRecord(after_k1, ctx->stream));
   if (!settle) return PXR_OK;
   for (;;) {     // window residency: whoever consumes these results right away needs them settled first
     int64_t n_fixed = 0;
@@ -1077,18 +1103,22 @@ int BA::inner_rounds(int set) {
   auto published = [&](int r) { return slots[3 * r + 2] == epoch; };
   InnerStepArgs a;
   a.n_points = n_points; a.point_off = point_off.p; a.pt_begin = pt_begin.p;
-  a.obs_out = obs_out.p; a.juv = juv.p; a.juv_stride = juv_stride; a.juv_w = 9 + K;
+  a.obs_out = obs_out.p; a.jpt = inner_jpt.p;
   a.xyz = X[set].p; a.st = inner_state.p;
   a.loss.type = opt.loss_type; a.loss.a = opt.loss_scale;
   a.epoch = epoch;
   const unsigned pgrid = (unsigned)cdiv(n_points, 128);
-  const unsigned sgrid = (unsigned)std::min<int64_t>(pgrid, (int64_t)ctx->sm_count * 8);
+  // Round r's lists are a subset of round r-2's, so the lengths that round published bound K0's and the step kernel's
+  // grids (both read the exact length on the device); before any round has published, n_obs / n_points do.
+  int64_t bound_obs = n_obs, bound_pts = n_points;
   if (time_inner_rounds && inner_round_timed.empty()) {
-    inner_round_timed.resize(kInnerRounds, {nullptr, nullptr});
-    for (auto& pr : inner_round_timed) { PXR_CUDA(cudaEventCreate(&pr.first)); PXR_CUDA(cudaEventCreate(&pr.second)); }
+    inner_round_timed.resize(kInnerRounds, {nullptr, nullptr, nullptr, nullptr});
+    for (auto& ev : inner_round_timed)
+      for (cudaEvent_t& e : ev) PXR_CUDA(cudaEventCreate(&e));
   }
   inner_rounds_timed = time_inner_rounds;
   inner_rounds_run = 0;
+  cap_plist.clear(); cap_list.clear(); cap_active.clear();
   PXR_CUDA(cudaMemsetAsync(inner_counters.p, 0, 6 * sizeof(unsigned long long), s));
   a.plist_next = inner_plist[0].p; a.list_next = inner_list[0].p; a.cnt_next = inner_counters.p;
   PXR_LAUNCH(ctx, inner_list_kernel, pgrid, 128, 0, a);
@@ -1107,21 +1137,55 @@ int BA::inner_rounds(int set) {
           std::this_thread::yield();
         }
       }
-      if (published(r2) && slots[3 * r2] == 0) break;
+      if (published(r2)) {
+        if (slots[3 * r2] == 0) break;
+        bound_obs = std::min<int64_t>(bound_obs, (int64_t)slots[3 * r2]);
+        bound_pts = std::min<int64_t>(bound_pts, (int64_t)slots[3 * r2 + 1]);
+      }
     }
     const int cur = round & 1;
     unsigned long long* cnt = inner_counters.p + 2 * (round % 3);
+    if (capture_inner_lists) PXR_TRY(capture_round_lists(inner_plist[cur].p, inner_list[cur].p, cnt));
     a.plist = inner_plist[cur].p; a.cnt = cnt;
     a.plist_next = inner_plist[1 - cur].p; a.list_next = inner_list[1 - cur].p;
     a.cnt_next = inner_counters.p + 2 * ((round + 1) % 3); a.cnt_clear = inner_counters.p + 2 * ((round + 2) % 3);
     a.publish = inner_cnt_dev + 3 * round;
-    if (inner_rounds_timed) PXR_CUDA(cudaEventRecord(inner_round_timed[round].first, s));
-    PXR_TRY(eval_list(set, inner_list[cur].p, n_obs, cnt, false));
+    cudaEvent_t* ev = inner_rounds_timed ? inner_round_timed[round].data() : nullptr;
+    if (ev) PXR_CUDA(cudaEventRecord(ev[0], s));
+    PXR_TRY(eval_list(set, inner_list[cur].p, n_obs, cnt, false, ev ? ev[1] : nullptr, ev ? ev[2] : nullptr, bound_obs));
+    const unsigned sgrid = (unsigned)std::min<int64_t>(cdiv(bound_pts, 128), (int64_t)ctx->sm_count * 8);
     PXR_LAUNCH(ctx, inner_step_kernel, sgrid, 128, 0, a, round == 0 ? 0 : 1);
-    if (inner_rounds_timed) PXR_CUDA(cudaEventRecord(inner_round_timed[round].second, s));
+    if (ev) PXR_CUDA(cudaEventRecord(ev[3], s));
+    if (capture_inner_lists) PXR_TRY(capture_round_active());
     inner_rounds_run = round + 1;
   }
   PXR_CUDA(cudaGetLastError());
+  return PXR_OK;
+}
+
+// pxr_ba_debug_inner_capture: a round's point and observation lists as the round starts (synchronous, tests only)
+int BA::capture_round_lists(const int64_t* plist, const int64_t* list, const unsigned long long* cnt) {
+  cudaStream_t s = ctx->stream;
+  unsigned long long c[2] = {0, 0};
+  PXR_CUDA(cudaMemcpyAsync(c, cnt, sizeof(c), cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  cap_list.emplace_back((size_t)c[0]); cap_plist.emplace_back((size_t)c[1]);
+  if (c[0]) PXR_CUDA(cudaMemcpyAsync(cap_list.back().data(), list, (size_t)c[0] * 8, cudaMemcpyDeviceToHost, s));
+  if (c[1]) PXR_CUDA(cudaMemcpyAsync(cap_plist.back().data(), plist, (size_t)c[1] * 8, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  return PXR_OK;
+}
+
+// ... and, after the round's step kernel, whether each of its points stays active
+int BA::capture_round_active() {
+  cudaStream_t s = ctx->stream;
+  std::vector<int32_t> act((size_t)n_points);
+  PXR_CUDA(cudaMemcpy2DAsync(act.data(), sizeof(int32_t), reinterpret_cast<const char*>(inner_state.p) + offsetof(InnerState, active),
+                             sizeof(InnerState), sizeof(int32_t), (size_t)n_points, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  const std::vector<int64_t>& pl = cap_plist.back();
+  cap_active.emplace_back(pl.size());
+  for (size_t i = 0; i < pl.size(); ++i) cap_active.back()[i] = act[(size_t)pl[i]] != 0 ? 1 : 0;
   return PXR_OK;
 }
 
@@ -1132,6 +1196,7 @@ int BA::inner_iterations_batched(int set) {
   if (!inner_state.p) {
     PXR_TRY(inner_state.alloc(n_points));
     for (int k = 0; k < 2; ++k) { PXR_TRY(inner_list[k].alloc(n_obs)); PXR_TRY(inner_plist[k].alloc(n_points)); }
+    PXR_TRY(alloc_inner_jpt());
     PXR_TRY(inner_counters.alloc(6));
     PXR_CUDA(cudaHostAlloc((void**)&inner_cnt_host, (size_t)kInnerRounds * 3 * sizeof(unsigned long long), cudaHostAllocMapped));
     std::memset(inner_cnt_host, 0, (size_t)kInnerRounds * 3 * sizeof(unsigned long long));
@@ -1826,6 +1891,7 @@ int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count
   DevBuf<unsigned long long> dn;
   if (n > 0) PXR_TRY(dlist.upload(list, (size_t)n, s));
   PXR_CUDA(cudaMemsetAsync(b->obs_out.p, 0xff, (size_t)b->n_obs * 64, s));
+  PXR_TRY(b->alloc_inner_jpt());
   if (count_on_device) {
     const unsigned long long hn = (unsigned long long)n;
     PXR_TRY(dn.upload(&hn, 1, s));
@@ -1835,6 +1901,64 @@ int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count
   }
   PXR_CUDA(cudaMemcpyAsync(out, b->obs_out.p, (size_t)b->n_obs * 64, cudaMemcpyDeviceToHost, s));
   PXR_CUDA(cudaStreamSynchronize(s));
+  return PXR_OK;
+}
+
+// The point-only K0 of the inner-iteration rounds next to the full K0 (tests), at the current parameters: uv_full
+// [n_obs][2] from the full projection over all observations, then uv [n_obs][2] and jpt [n_obs][6] (d(uv)/dX, rows u
+// then v) from the point-only one over list[0..n), NaN outside the list.  count_on_device as in pxr_ba_debug_eval_list.
+int pxr_ba_debug_project_point(pxr_ba* ba, const int64_t* list, int64_t n, int count_on_device, double* uv, double* jpt,
+                               double* uv_full) {
+  if (!ba || n < 0 || (n > 0 && !list) || !uv || !jpt || !uv_full) return fail(PXR_ERR_INVALID_ARGUMENT, "bad arguments");
+  BA* b = reinterpret_cast<BA*>(ba);
+  pxr_ctx* ctx = b->ctx;
+  cudaStream_t s = ctx->stream;
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  if (n > b->n_obs) return fail(PXR_ERR_INVALID_ARGUMENT, "a list holds at most n_obs entries");
+  for (int64_t i = 0; i < n; ++i)
+    if (list[i] < 0 || list[i] >= b->n_obs) return fail(PXR_ERR_INVALID_ARGUMENT, "list entry out of range");
+  DevBuf<int64_t> dlist;
+  DevBuf<unsigned long long> dn;
+  if (n > 0) PXR_TRY(dlist.upload(list, (size_t)n, s));
+  PXR_TRY(b->project(b->cur, true, nullptr));
+  PXR_CUDA(cudaMemcpyAsync(uv_full, b->uv.p, (size_t)b->n_obs * 16, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaMemsetAsync(b->uv.p, 0xff, (size_t)b->n_obs * 16, s));
+  PXR_TRY(b->alloc_inner_jpt());
+  PXR_CUDA(cudaMemsetAsync(b->inner_jpt.p, 0xff, (size_t)b->n_obs * 48, s));
+  if (count_on_device) {
+    const unsigned long long hn = (unsigned long long)n;
+    PXR_TRY(dn.upload(&hn, 1, s));
+    PXR_TRY(b->project_point_list(b->cur, dlist.p, b->n_obs, dn.p, b->n_obs));
+  } else {
+    PXR_TRY(b->project_point_list(b->cur, dlist.p, n, nullptr, n));
+  }
+  PXR_CUDA(cudaMemcpyAsync(uv, b->uv.p, (size_t)b->n_obs * 16, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaMemcpyAsync(jpt, b->inner_jpt.p, (size_t)b->n_obs * 48, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  return PXR_OK;
+}
+
+int pxr_ba_debug_inner_capture(pxr_ba* ba, int enable) {
+  if (!ba) return fail(PXR_ERR_INVALID_ARGUMENT, "ba is NULL");
+  reinterpret_cast<BA*>(ba)->capture_inner_lists = enable != 0;
+  return PXR_OK;
+}
+
+// Round `round` of the most recent batched inner iterations run with capture on (tests): *n_points / *n_obs are its list
+// lengths; plist / list / active (each may be NULL) receive its point list, its observation list and, per listed point,
+// whether the round's step kernel kept it active.
+int pxr_ba_debug_inner_round_lists(pxr_ba* ba, int round, int64_t* plist, int64_t* list, uint8_t* active, int64_t* n_points,
+                                   int64_t* n_obs) {
+  if (!ba) return fail(PXR_ERR_INVALID_ARGUMENT, "ba is NULL");
+  BA* b = reinterpret_cast<BA*>(ba);
+  if (round < 0 || round >= (int)b->cap_active.size()) return fail(PXR_ERR_INVALID_ARGUMENT, "round %d was not captured", round);
+  const std::vector<int64_t>& pl = b->cap_plist[round];
+  const std::vector<int64_t>& ol = b->cap_list[round];
+  if (n_points) *n_points = (int64_t)pl.size();
+  if (n_obs) *n_obs = (int64_t)ol.size();
+  if (plist) std::copy(pl.begin(), pl.end(), plist);
+  if (list) std::copy(ol.begin(), ol.end(), list);
+  if (active) std::copy(b->cap_active[round].begin(), b->cap_active[round].end(), active);
   return PXR_OK;
 }
 
@@ -1876,11 +2000,31 @@ int pxr_ba_debug_inner_rounds(pxr_ba* ba, int enable_timing, int capacity, unsig
     if (ms) {
       float t = -1.f;
       if (b->inner_rounds_timed)
-        PXR_CUDA(cudaEventElapsedTime(&t, b->inner_round_timed[r].first, b->inner_round_timed[r].second));
+        PXR_CUDA(cudaEventElapsedTime(&t, b->inner_round_timed[r][0], b->inner_round_timed[r][3]));
       ms[r] = t;
     }
   }
   if (enable_timing >= 0) b->time_inner_rounds = enable_timing != 0;
+  return PXR_OK;
+}
+
+// The per-launch split of those rounds (profiling): ms[3r] from the round's start to the end of K0, ms[3r+1] from
+// there to the end of K1, ms[3r+2] from there to the end of the step kernel (-1 where round timing was off).  Each part
+// is stream time, so it includes the launch gap in front of its kernel.
+int pxr_ba_debug_inner_round_split(pxr_ba* ba, int capacity, double* ms, int* n_rounds) {
+  if (!ba || capacity < 0 || (capacity > 0 && !ms)) return fail(PXR_ERR_INVALID_ARGUMENT, "bad arguments");
+  BA* b = reinterpret_cast<BA*>(ba);
+  PXR_CUDA(cudaSetDevice(b->ctx->device));
+  PXR_CUDA(cudaStreamSynchronize(b->ctx->stream));
+  const int n = b->inner_cnt_host ? b->inner_rounds_run : 0;
+  if (n_rounds) *n_rounds = n;
+  for (int r = 0; r < std::min(n, capacity); ++r)
+    for (int k = 0; k < 3; ++k) {
+      float t = -1.f;
+      if (b->inner_rounds_timed)
+        PXR_CUDA(cudaEventElapsedTime(&t, b->inner_round_timed[r][k], b->inner_round_timed[r][k + 1]));
+      ms[3 * r + k] = t;
+    }
   return PXR_OK;
 }
 

@@ -1,5 +1,6 @@
 // pxr_ba_host.h — host-side state of one featuremetric BA problem resident on the device.
 #pragma once
+#include <array>
 #include <cstdlib>
 #include <chrono>
 #include <string>
@@ -184,7 +185,7 @@ struct BA {
   DevBuf<int64_t> io_chunk_begin; int64_t io_n_chunks = 0;
   DevBuf<long long> chol_trace;     // PXR_CHOL_TRACE=<file>: panel-CTA time stamps
   DevBuf<int> chol_sync;            // flags of the persistent tile-DAG Cholesky (pxr_chol.cuh)
-  void clear_inner_round_timing() { for (auto& pr : inner_round_timed) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); } inner_round_timed.clear(); }
+  void clear_inner_round_timing() { for (auto& ev : inner_round_timed) for (cudaEvent_t e : ev) cudaEventDestroy(e); inner_round_timed.clear(); }
   ~BA() { if (inner_cnt_host) cudaFreeHost(inner_cnt_host); clear_inner_round_timing(); if (res_thread.joinable()) res_thread.join(); if (chol_graph_exec) cudaGraphExecDestroy(chol_graph_exec); for (int k = 0; k < kNumStages; ++k) for (auto& pr : timed[k]) { cudaEventDestroy(pr.first); cudaEventDestroy(pr.second); } }
   // static co-visibility structure for the Schur complement (see ba_schur_pairs_kernel)
   DevBuf<int32_t> sp_px, sp_py, sp_pp;
@@ -237,7 +238,15 @@ struct BA {
   int gradient_max_norm(double* out);
   int inner_iterations(int set);
   int inner_iterations_batched(int set);
-  int eval_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev = nullptr, bool settle = true);
+  int eval_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev = nullptr, bool settle = true,
+                cudaEvent_t after_k0 = nullptr, cudaEvent_t after_k1 = nullptr, int64_t k0_bound = -1);
+  int alloc_inner_jpt();                            // inner_jpt's one allocation: before the rounds, or a debug entry
+  bool capture_inner_lists = false;                // pxr_ba_debug_inner_capture: keep every round's lists (synchronous)
+  std::vector<std::vector<int64_t>> cap_plist, cap_list;
+  std::vector<std::vector<uint8_t>> cap_active;
+  int capture_round_lists(const int64_t* plist, const int64_t* list, const unsigned long long* cnt);
+  int capture_round_active();
+  int project_point_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev, int64_t grid_bound);
   int inner_rounds(int set);                       // the <= 52 rounds of inner_iterations_batched, without a host wait per round
   unsigned long long* inner_cnt_host = nullptr;    // pinned, mapped [kInnerRounds][3]: each round's list lengths + the epoch of the call
   unsigned long long* inner_cnt_dev = nullptr;     // the same slots, device view (written by inner_step_kernel)
@@ -245,11 +254,12 @@ struct BA {
   int inner_rounds_run = 0;                        // rounds enqueued by the most recent inner_rounds (profiling)
   bool time_inner_rounds = false;                  // pxr_ba_debug_inner_rounds: stream time of every round of the next calls
   bool inner_rounds_timed = false;                 // the most recent inner_rounds call recorded them
-  std::vector<std::pair<cudaEvent_t, cudaEvent_t>> inner_round_timed;
+  std::vector<std::array<cudaEvent_t, 4>> inner_round_timed;   // per round: before K0, after K0, after K1, after the step kernel
   DevBuf<double> inner_snapshot;                   // window residency: the points before a batch of rounds (redo after a refetch)
   DevBuf<InnerState> inner_state;
   DevBuf<int64_t> inner_list[2], inner_plist[2];   // a round's observation / point lists, alternating between rounds
   DevBuf<unsigned long long> inner_counters;       // 3 x [observations, points], rotating
+  DevBuf<double> inner_jpt;                        // [n_obs][6]: d(uv)/dX of the observations a round evaluated
   bool use_monolithic_inner = false;
   int step_norm_between_sets(double* out);
   int lm_begin();

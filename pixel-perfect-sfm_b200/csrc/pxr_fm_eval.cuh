@@ -35,6 +35,7 @@ struct ProjectArgs {
   double* juv;   // optional [n_obs][juv_stride]: 2 x (6 pose | 3 point | K intr), row-major
   int juv_stride;
   int juv_k;     // K columns stored per row
+  double* jpt = nullptr;   // ba_project_point_kernel: [n_obs][6] d(uv)/dX, rows u then v (the point columns of juv)
 };
 
 // one observation: uv (and xy) to global memory, the 2 x (9 + K) record d(uv)/d(theta) to `out` (global or shared)
@@ -80,6 +81,29 @@ __global__ void __launch_bounds__(128) ba_project_kernel(ProjectArgs a) {
   for (int64_t k = a.obs_begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < end; k += (int64_t)gridDim.x * blockDim.x) {
     const int64_t o = a.item_index ? a.item_index[k] : k;
     project_observation<JAC>(a, o, (JAC && a.juv) ? a.juv + o * (int64_t)a.juv_stride : nullptr);
+  }
+}
+
+// Point-only variant for the inner-iteration rounds, whose step kernel reads nothing of the record but d(uv)/dX: uv (and
+// xy) as above and the 2 x 3 point block to the compact `jpt` ([n_obs][6], rows u then v), 48 B per observation instead
+// of 2 x (9 + K) strided doubles in `juv`.  The whole record is still formed, into the thread's row of shared memory as
+// ba_project_staged_kernel does: left with nothing to store, the compiler would drop the pose and intrinsics columns
+// and could then contract the shared subexpressions differently, and the point columns must be the full K0's bit for
+// bit.  Dynamic shared memory: 128 * (juv_stride | 1) doubles, within the 48 KiB a launch gets without an opt-in.
+static_assert(128 * ((2 * (9 + kMaxK)) | 1) * sizeof(double) <= 48 * 1024,
+              "ba_project_point_kernel's shared rows need the dynamic shared memory opt-in");
+static __global__ void __launch_bounds__(128) ba_project_point_kernel(ProjectArgs a) {
+  extern __shared__ double sm_proj[];
+  const int W = 9 + a.juv_k;
+  double* row = sm_proj + threadIdx.x * (a.juv_stride | 1);
+  const int64_t end = a.n_dev ? a.obs_begin + (int64_t)*a.n_dev : a.obs_end;
+  for (int64_t k = a.obs_begin + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < end; k += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t o = a.item_index ? a.item_index[k] : k;
+    project_observation<true>(a, o, row);
+    double2* out = reinterpret_cast<double2*>(a.jpt + 6 * o);
+    out[0] = make_double2(row[6], row[7]);
+    out[1] = make_double2(row[8], row[W + 6]);
+    out[2] = make_double2(row[W + 7], row[W + 8]);
   }
 }
 

@@ -225,7 +225,7 @@ struct InnerState {
 struct InnerStepArgs {
   int64_t n_points;
   const int64_t* point_off; const int64_t* pt_begin;
-  const double* obs_out; const double* juv; int juv_stride; int juv_w;  // juv_w = 9 + K
+  const double* obs_out; const double* jpt;   // K1's records and K0's d(uv)/dX ([n_obs][6]) of the round's observations
   double* xyz;          // candidate parameter set
   InnerState* st;
   LossParams loss;
@@ -284,6 +284,8 @@ __device__ __forceinline__ bool inner_propose(InnerState& s) {
   }
 }
 
+constexpr int kInnerBatch = 4;   // observation records a step-kernel thread loads ahead of its serial sum
+
 // phase 0: state from the evaluation at the start point; phase 1: judge the evaluated candidate
 // returns whether point p stays active (proposes another candidate)
 __device__ __forceinline__ bool inner_step_point(const InnerStepArgs& a, int64_t p, int phase) {
@@ -295,28 +297,44 @@ __device__ __forceinline__ bool inner_step_point(const InnerStepArgs& a, int64_t
 #pragma unroll
     for (int k = 0; k < 3; ++k) s.x[k] = a.xyz[3 * p + k];
   } else if (!s.active) return false;
-  // cost / J^T J / J^T r of this point at the evaluated location
+  // cost / J^T J / J^T r of this point at the evaluated location, summed serially in observation order.  The records of
+  // up to kInnerBatch observations are loaded ahead of the sum, so their loads are in flight together.
   double cost = 0, H[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0};
-  for (int64_t o = a.pt_begin[p]; o < a.pt_begin[p + 1]; ++o) {
-    const double* oo = a.obs_out + o * 8;
-    double rho[3];
-    loss_eval(a.loss, 1.0, oo[0], rho);
-    cost += 0.5 * rho[0];
-    const double bu = rho[1] * oo[1], bv = rho[1] * oo[2];
-    const double auu = rho[1] * oo[3], auv = rho[1] * oo[4], avv = rho[1] * oo[5];
-    const double* J = a.juv + o * (int64_t)a.juv_stride;
-    const double pu[3] = {J[6], J[7], J[8]}, pv[3] = {J[a.juv_w + 6], J[a.juv_w + 7], J[a.juv_w + 8]};
-    double apu[3], apv[3];
+  const int64_t ob = a.pt_begin[p], oe = a.pt_begin[p + 1];
+  for (int64_t o0 = ob; o0 < oe; o0 += kInnerBatch) {
+    const int nb = (int)min((int64_t)kInnerBatch, oe - o0);
+    double2 rec[kInnerBatch][3], jac[kInnerBatch][3];
 #pragma unroll
-    for (int k = 0; k < 3; ++k) { apu[k] = auu * pu[k] + auv * pv[k]; apv[k] = auv * pu[k] + avv * pv[k]; }
-    H[0] += pu[0] * apu[0] + pv[0] * apv[0];
-    H[1] += pu[0] * apu[1] + pv[0] * apv[1];
-    H[2] += pu[0] * apu[2] + pv[0] * apv[2];
-    H[3] += pu[1] * apu[1] + pv[1] * apv[1];
-    H[4] += pu[1] * apu[2] + pv[1] * apv[2];
-    H[5] += pu[2] * apu[2] + pv[2] * apv[2];
+    for (int b = 0; b < kInnerBatch; ++b) {
+      if (b < nb) {
+        const double2* oo = reinterpret_cast<const double2*>(a.obs_out + (o0 + b) * 8);
+        const double2* jj = reinterpret_cast<const double2*>(a.jpt + (o0 + b) * 6);
 #pragma unroll
-    for (int k = 0; k < 3; ++k) g[k] += pu[k] * bu + pv[k] * bv;
+        for (int k = 0; k < 3; ++k) { rec[b][k] = oo[k]; jac[b][k] = jj[k]; }
+      }
+    }
+#pragma unroll
+    for (int b = 0; b < kInnerBatch; ++b) {
+      if (b >= nb) break;
+      const double oo[6] = {rec[b][0].x, rec[b][0].y, rec[b][1].x, rec[b][1].y, rec[b][2].x, rec[b][2].y};
+      double rho[3];
+      loss_eval(a.loss, 1.0, oo[0], rho);
+      cost += 0.5 * rho[0];
+      const double bu = rho[1] * oo[1], bv = rho[1] * oo[2];
+      const double auu = rho[1] * oo[3], auv = rho[1] * oo[4], avv = rho[1] * oo[5];
+      const double pu[3] = {jac[b][0].x, jac[b][0].y, jac[b][1].x}, pv[3] = {jac[b][1].y, jac[b][2].x, jac[b][2].y};
+      double apu[3], apv[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { apu[k] = auu * pu[k] + auv * pv[k]; apv[k] = auv * pu[k] + avv * pv[k]; }
+      H[0] += pu[0] * apu[0] + pv[0] * apv[0];
+      H[1] += pu[0] * apu[1] + pv[0] * apv[1];
+      H[2] += pu[0] * apu[2] + pv[0] * apv[2];
+      H[3] += pu[1] * apu[1] + pv[1] * apv[1];
+      H[4] += pu[1] * apu[2] + pv[1] * apv[2];
+      H[5] += pu[2] * apu[2] + pv[2] * apv[2];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) g[k] += pu[k] * bu + pv[k] * bv;
+    }
   }
   const double ftol = 1e-6, ptol = 1e-8, min_rel_dec = 1e-3, max_radius = 1e16;
   bool go = true;
@@ -368,6 +386,41 @@ __device__ __forceinline__ bool inner_step_point(const InnerStepArgs& a, int64_t
   return go;
 }
 
+// The next round's lists from one warp: lane i holds point p (when `stays`).  One atomic per counter per warp; the
+// warp's points land in lane order, and their observations, each point's in pt_begin order, are written by the whole
+// warp with consecutive stores.  Every lane of the warp must call this.
+__device__ __forceinline__ void inner_append(const InnerStepArgs& a, bool stays, int64_t p) {
+  const int lane = threadIdx.x & 31;
+  const unsigned mask = __ballot_sync(0xffffffffu, stays);
+  if (!mask) return;
+  int64_t ob = 0, no = 0;
+  if (stays) { ob = a.pt_begin[p]; no = a.pt_begin[p + 1] - ob; }
+  int64_t inc = no;   // inclusive scan of the observation counts over the lanes
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const int64_t t = __shfl_up_sync(0xffffffffu, inc, d);
+    if (lane >= d) inc += t;
+  }
+  const int64_t total = __shfl_sync(0xffffffffu, inc, 31), exc = inc - no;
+  unsigned long long obase = 0, pbase = 0;
+  if (lane == 0) {
+    obase = atomicAdd(&a.cnt_next[0], (unsigned long long)total);
+    pbase = atomicAdd(&a.cnt_next[1], (unsigned long long)__popc(mask));
+  }
+  obase = __shfl_sync(0xffffffffu, obase, 0);
+  pbase = __shfl_sync(0xffffffffu, pbase, 0);
+  if (stays) a.plist_next[pbase + __popc(mask & ((1u << lane) - 1u))] = p;
+  for (int64_t j0 = 0; j0 < total; j0 += 32) {
+    const int64_t j = j0 + lane;
+    int src = 0;   // the last lane whose observations start at or before entry j (lanes with no observations are skipped
+#pragma unroll    // over: they share their start with the next lane that has some)
+    for (int step = 16; step > 0; step >>= 1)
+      if (__shfl_sync(0xffffffffu, exc, src + step) <= j) src += step;
+    const int64_t sob = __shfl_sync(0xffffffffu, ob, src), sexc = __shfl_sync(0xffffffffu, exc, src);
+    if (j < total) a.list_next[obase + j] = sob + (j - sexc);
+  }
+}
+
 static __global__ void __launch_bounds__(128) inner_step_kernel(InnerStepArgs a, int phase) {
   const unsigned long long n = a.cnt[1];
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -376,27 +429,23 @@ static __global__ void __launch_bounds__(128) inner_step_kernel(InnerStepArgs a,
     __threadfence_system();
     *(volatile unsigned long long*)(a.publish + 2) = a.epoch;
   }
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const int64_t p = a.plist[i];
-    if (!inner_step_point(a, p, phase)) continue;
-    const int64_t ob = a.pt_begin[p], no = a.pt_begin[p + 1] - ob;
-    const unsigned long long base = atomicAdd(&a.cnt_next[0], (unsigned long long)no);
-    a.plist_next[atomicAdd(&a.cnt_next[1], 1ull)] = p;
-    for (int64_t k = 0; k < no; ++k) a.list_next[base + k] = ob + k;
+  // warp-uniform trip count: the whole warp takes part in inner_append
+  const uint64_t lane = threadIdx.x & 31;
+  for (uint64_t w = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x - lane; w < n; w += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t i = w + lane;
+    int64_t p = -1;
+    bool stays = false;
+    if (i < n) { p = a.plist[i]; stays = inner_step_point(a, p, phase); }
+    inner_append(a, stays, p);
   }
 }
 
 // round 0's lists: every variable point with observations, and those observations
 static __global__ void __launch_bounds__(128) inner_list_kernel(InnerStepArgs a) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= a.n_points) return;
-  if (!(a.point_off[p] >= 0 && a.pt_begin[p + 1] > a.pt_begin[p])) return;
-  const int64_t ob = a.pt_begin[p], n = a.pt_begin[p + 1] - ob;
-  const unsigned long long base = atomicAdd(&a.cnt_next[0], (unsigned long long)n);
-  a.plist_next[atomicAdd(&a.cnt_next[1], 1ull)] = p;
-  for (int64_t i = 0; i < n; ++i) a.list_next[base + i] = ob + i;
+  const bool listed = p < a.n_points && a.point_off[p] >= 0 && a.pt_begin[p + 1] > a.pt_begin[p];
+  inner_append(a, listed, p);
 }
-
 
 // ||a - b|| over two parameter sets (ambient), for step_norm after inner iterations
 static __global__ void __launch_bounds__(256) diff_norm_kernel(const double* a, const double* b, int64_t n, double* acc, double* part = nullptr) {

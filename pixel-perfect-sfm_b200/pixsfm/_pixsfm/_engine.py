@@ -87,6 +87,33 @@ class BAHandle:
                                                     int(bool(count_on_device)), _p(out)))
         return out
 
+    def debug_project_point(self, items, count_on_device=False):
+        """the rounds' point-only projection over the observation list `items` next to the full one: uv [n_obs, 2] and
+        jpt [n_obs, 2, 3] (d(uv)/dX, NaN rows outside the list) and uv_full [n_obs, 2] of the full projection"""
+        items = np.ascontiguousarray(items, np.int64)
+        n = self.problem.n_obs
+        uv, jpt, uv_full = np.empty((n, 2)), np.empty((n, 2, 3)), np.empty((n, 2))
+        _capi.check(self.lib.pxr_ba_debug_project_point(self.handle, _p(items), C.c_int64(len(items)),
+                                                        int(bool(count_on_device)), _p(uv), _p(jpt), _p(uv_full)))
+        return dict(uv=uv, jpt=jpt, uv_full=uv_full)
+
+    def debug_inner_capture(self, enable=True):
+        """keep every round's lists in the batched inner iterations that follow (the host waits for every round)"""
+        _capi.check(self.lib.pxr_ba_debug_inner_capture(self.handle, int(bool(enable))))
+
+    def debug_inner_round_lists(self):
+        """the captured rounds of the most recent batched inner iterations: per round a dict of its point list, its
+        observation list and, per listed point, whether the round's step kernel kept it active"""
+        out = []
+        for r in range(10 ** 6):
+            npt, nob = C.c_int64(), C.c_int64()
+            if self.lib.pxr_ba_debug_inner_round_lists(self.handle, r, None, None, None, C.byref(npt), C.byref(nob)) != 0:
+                break
+            pl, ol, act = np.empty(npt.value, np.int64), np.empty(nob.value, np.int64), np.empty(npt.value, np.uint8)
+            _capi.check(self.lib.pxr_ba_debug_inner_round_lists(self.handle, r, _p(pl), _p(ol), _p(act), None, None))
+            out.append(dict(points=pl, obs=ol, active=act.astype(bool)))
+        return out
+
     def debug_eval_records(self, mode=1):
         """[n_obs, 8] per-observation K1 record after K0 + K1 over all observations, mode 0 (cost only: column 0, NaN
         elsewhere) or 1 (Jacobian)"""
@@ -102,6 +129,13 @@ class BAHandle:
                                                        C.byref(n)))
         k = min(n.value, capacity)
         return counts[:k], ms[:k]
+
+    def debug_inner_round_split(self, capacity=64):
+        """[n, 3] stream ms of each round of the most recent batched inner iterations, split at the ends of K0, K1 and the
+        step kernel (-1 where round timing was off during that call)"""
+        ms = np.zeros((capacity, 3)); n = C.c_int()
+        _capi.check(self.lib.pxr_ba_debug_inner_round_split(self.handle, int(capacity), _p(ms), C.byref(n)))
+        return ms[:min(n.value, capacity)]
 
     def solve(self, capacity=512):
         s = _capi.make_summary(capacity)

@@ -12,7 +12,9 @@ that trajectory twice from the same start:
      with its active points, active observations and stream time.  That is the time between two events recorded
      around the round's launches, so it includes any time the device sat idle waiting for the host to enqueue them
      (the host runs ahead of the device and only waits on a round two behind): it is not kernel time.  The extra
-     events make this pass slightly slower.
+     events make this pass slightly slower.  Each round is also split at the ends of its three launches
+     (pxr_ba_debug_inner_round_split): K0 (the projection), K1 (fm_eval_kernel) and the step kernel, each part with
+     the launch gap in front of it, reported per round and summed per LM iteration.
 It prints one JSON object, with the card name and power limit read in the same process, and the share of the inner
 rounds whose list is shorter than 32 items per K1 warp (--short-list, default 32 x 132 SMs x 16 warps = 67 584).
 """
@@ -92,10 +94,16 @@ def main():
         rounds = []
         if ran:
             counts, ms = h.debug_inner_rounds()
-            rounds = [{"active_obs": int(c[0]), "active_points": int(c[1]), "ms": float(t)} for c, t in zip(counts, ms)]
+            split = h.debug_inner_round_split()
+            rounds = [{"active_obs": int(c[0]), "active_points": int(c[1]), "ms": float(t),
+                       "k0_ms": float(sp[0]), "k1_ms": float(sp[1]), "step_ms": float(sp[2])}
+                      for c, t, sp in zip(counts, ms, split)]
         short = [r for r in rounds if r["active_obs"] < own.short_list]
         per_it.append(dict(stages[it], iteration=it, rounds=len(rounds),
                            rounds_ms=sum(r["ms"] for r in rounds),
+                           rounds_k0_ms=sum(r["k0_ms"] for r in rounds),
+                           rounds_k1_ms=sum(r["k1_ms"] for r in rounds),
+                           rounds_step_ms=sum(r["step_ms"] for r in rounds),
                            short_rounds=len(short), short_rounds_ms=sum(r["ms"] for r in short),
                            round_list=rounds))
     h.debug_inner_rounds(enable_timing=0)
