@@ -541,6 +541,79 @@ typedef struct {
 int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* desc, const pxr_interp_config* interp,
                const pxr_solver_options* opt, pxr_summary* summary);
 
+/* ---- batched query bundle adjustment ------------------------------------------
+ * replaces a loop of _localization.QueryBundleOptimizer.run (localization/bindings.cc;
+ * single_query_bundle_optimizer.h, query_bundle_optimizer.h SolveProblem): N independent queries, each one image's
+ * pose (QuaternionManifold rotation + translation) and optionally some of its camera's intrinsics, refined against
+ * fixed 3D points and fixed fp64 reference descriptors.  One CTA solves one query end to end (csrc/pxr_qba.cu); every
+ * per-query decision is the one pxr_ba_run takes on that query alone (one free image, constant points, no inner
+ * iterations).  A query's results do not depend on which other queries share its launch. */
+typedef struct {
+  int32_t n_queries;
+  /* per query */
+  const int32_t* cam_model;       /* [n_queries] pxr_camera_model */
+  double* cam_params;             /* [n_queries][PXR_MAX_CAM_PARAMS] in/out */
+  const uint32_t* cam_const_mask; /* [n_queries] bit i: param i constant; 0xFFFFFFFF: camera constant */
+  double* qvec;                   /* [n_queries][4] in/out (w,x,y,z), world->camera */
+  double* tvec;                   /* [n_queries][3] in/out */
+  const int64_t* obs_begin;       /* [n_queries+1] non-decreasing: query q owns residual blocks [obs_begin[q], obs_begin[q+1]) */
+  /* per residual block (a correspondence compared with several descriptors gives several blocks) */
+  const double* xyz;              /* [n_obs][3] constant 3D point */
+  const int64_t* obs_patch;       /* [n_obs] patch index within its query's patch block */
+  const double* refs;             /* [n_obs][channels] fixed reference descriptor */
+  /* patches: one block per query, [patch_counts[q]][ph][pw][channels], each in host OR device memory (a device block is
+   * read in place, never copied) */
+  const void* const* patch_blocks;   /* [n_queries] */
+  const int64_t* patch_counts;       /* [n_queries] */
+  const int32_t* corner;          /* [sum patch_counts][2] (x0,y0), query blocks back to back */
+  const double* scale;            /* [sum patch_counts][2] */
+  double upsampling_factor;
+  int32_t ph, pw, channels, patch_dtype;
+  /* bytes a wave may upload (host patch blocks, descriptors, points, per-query state); 0: half of the free device
+   * memory at the call */
+  double max_wave_bytes;
+} pxr_qba_desc;
+
+typedef struct {
+  int32_t status;                 /* PXR_OK, or PXR_ERR_NUMERIC: initial cost not finite (parameters untouched) */
+  int32_t num_residual_blocks;    /* 0: not solved, parameters untouched */
+  double initial_cost;
+  double final_cost;              /* cost of the parameters written back (the lowest-cost iterate) */
+  int32_t num_iterations;         /* iteration summaries recorded, as pxr_summary::num_iterations */
+  int32_t num_successful_steps;
+  int32_t num_unsuccessful_steps;
+  int32_t termination_type;       /* as pxr_summary */
+  int64_t block_evaluations;      /* residual-block evaluations the kernel ran (blocks x passes) */
+} pxr_qba_result;
+
+/* Solves every query and writes the refined qvec / tvec / cam_params back into the desc arrays.
+ *  results     [n_queries]
+ *  iterations  [n_queries][iterations_capacity] or NULL: per-query iteration summaries (iteration_time_s is 0)
+ *  n_waves     or NULL: launches made (one per wave)
+ *  total       or NULL: h2d_bytes, kernel_launches, solve and total time, summed costs / steps, message
+ * Options: use_inner_iterations must be 0 (PXR_ERR_INVALID_ARGUMENT: no free points), ITERATIVE_SCHUR is
+ * PXR_ERR_UNSUPPORTED, `deterministic` is accepted and changes nothing (the path always sums in a fixed order).
+ * Queries are packed in order into waves of at most max_wave_bytes uploaded bytes (a larger query gets a wave of its
+ * own); the next wave's upload runs while the current one solves (two wave buffers when both fit in free device
+ * memory, else one, reused once the previous wave's outputs are back), and the interrupt callback is polled between
+ * waves.
+ * Arguments are checked before the context: a NULL or malformed desc is reported without a device. */
+int pxr_qba_run(pxr_ctx* ctx, const pxr_qba_desc* desc, const pxr_interp_config* interp, const pxr_solver_options* opt,
+                pxr_qba_result* results, pxr_iteration_summary* iterations, int32_t iterations_capacity, int32_t* n_waves,
+                pxr_summary* total);
+/* The wave plan pxr_qba_run uses: wave_begin [n_queries+1] receives the first query of every wave (entries past
+ * *n_waves are left alone), wave_bytes [n_queries] (or NULL) each wave's upload.  Host computation with two device
+ * queries: with max_wave_bytes 0 the budget is half of the free device memory (PXR_ERR_NO_DEVICE without a device),
+ * and each patch block's placement is asked from the CUDA runtime (a block it cannot place counts as host memory). */
+int pxr_qba_plan_waves(const pxr_qba_desc* desc, int32_t* wave_begin, int32_t* n_waves, double* wave_bytes);
+/* Evaluates every query at the given parameters with the solver's device code and moves nothing (tests).
+ *  cost [n_queries]; H [n_queries][18][18] the lower triangle of J^T J in the query's tangent columns (3 rotation,
+ *  3 translation, then the free intrinsics in parameter order; the rest 0); g [n_queries][18] J^T r;
+ *  xy [n_obs][2] projected image point; rec [n_obs][8] s, G^T r (2), G^T G (3), 0, 0 as pxr_ba_evaluate.  Any output
+ *  may be NULL.  All queries run in one launch. */
+int pxr_qba_debug_linearize(pxr_ctx* ctx, const pxr_qba_desc* desc, const pxr_interp_config* interp,
+                            const pxr_solver_options* opt, double* cost, double* H, double* g, double* xy, double* rec);
+
 /* ---- host-side integer algorithms (bit-exact targets) -------------------
  * replace _base.compute_track_labels / compute_score_labels / compute_root_labels
  * (base/src/graph.cc:126-256) and keypoint_adjustment/main.py:13-57 find_problem_labels. */

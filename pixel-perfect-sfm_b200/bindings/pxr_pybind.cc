@@ -315,6 +315,69 @@ PYBIND11_MODULE(_pxr_pybind, m) {
     check(rc);
     return summary_dict(s, its);
   }, "ctx"_a, "problem"_a, "options"_a = py::dict());
+  // batched query BA (a loop of QueryBundleOptimizer.run): per query cam_model, cam_params [nq,12] / qvec [nq,4] /
+  // tvec [nq,3] (refined IN PLACE), cam_const_mask, obs_begin [nq+1]; per residual block xyz, obs_patch, refs;
+  // `patch_blocks` one host [n_q,H,W,C] array per query, `corner` / `scale` of their patches back to back
+  m.def("qba_run", [](Context& ctx, py::dict problem, py::dict interpolation, py::dict options) {
+    Fields f{problem, {}};
+    pxr_qba_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.n_queries = (int32_t)f.len("cam_model");
+    d.cam_model = f.arr<int32_t>("cam_model");
+    d.cam_params = f.inout<double>("cam_params");
+    d.cam_const_mask = f.arr<uint32_t>("cam_const_mask");
+    d.qvec = f.inout<double>("qvec");
+    d.tvec = f.inout<double>("tvec");
+    d.obs_begin = f.arr<int64_t>("obs_begin");
+    if (f.len("obs_begin") != (int64_t)d.n_queries + 1) throw py::value_error("obs_begin must hold n_queries + 1 entries");
+    d.xyz = f.arr<double>("xyz", false);
+    d.obs_patch = f.arr<int64_t>("obs_patch", false);
+    d.refs = f.arr<double>("refs", false);
+    if (!problem.contains("patch_blocks")) throw py::value_error("missing field 'patch_blocks'");
+    py::list blocks = problem["patch_blocks"];
+    if ((int64_t)py::len(blocks) != d.n_queries) throw py::value_error("one patch block per query is required");
+    std::vector<const void*> ptrs;
+    std::vector<int64_t> counts;
+    for (auto item : blocks) {
+      py::array a = py::array::ensure(item);
+      if (!a || a.ndim() != 4 || !(a.flags() & py::array::c_style))
+        throw py::value_error("patch blocks must be C-contiguous [N,H,W,C] arrays");
+      f.keep.push_back(a);
+      if (ptrs.empty()) {
+        d.patch_dtype = dtype_id(a);
+        d.ph = (int32_t)a.shape(1); d.pw = (int32_t)a.shape(2); d.channels = (int32_t)a.shape(3);
+      } else if (dtype_id(a) != d.patch_dtype || a.shape(1) != d.ph || a.shape(2) != d.pw || a.shape(3) != d.channels) {
+        throw py::value_error("patch blocks must share one dtype and patch shape");
+      }
+      ptrs.push_back(a.data());
+      counts.push_back((int64_t)a.shape(0));
+    }
+    d.patch_blocks = ptrs.data();
+    d.patch_counts = counts.data();
+    d.corner = f.arr<int32_t>("corner", false);
+    d.scale = f.arr<double>("scale", false);
+    d.upsampling_factor = f.scalar<double>("upsampling_factor", 1.0);
+    d.max_wave_bytes = f.scalar<double>("max_wave_bytes", 0.0);
+    const pxr_interp_config ic = interp_config(interpolation);
+    pxr_solver_options so; pxr_default_ba_options(&so); so.use_inner_iterations = 0; apply_options(so, options);
+    std::vector<pxr_qba_result> res((size_t)std::max(d.n_queries, 1));
+    int32_t n_waves = 0;
+    pxr_summary s; std::memset(&s, 0, sizeof(s));
+    int rc;
+    { py::gil_scoped_release nogil; rc = pxr_qba_run(ctx.h, &d, &ic, &so, res.data(), nullptr, 0, &n_waves, &s); }
+    check(rc);
+    py::list out;
+    for (int q = 0; q < d.n_queries; ++q) {
+      const pxr_qba_result& r = res[q];
+      out.append(py::dict("status"_a = r.status, "num_residual_blocks"_a = r.num_residual_blocks,
+                          "initial_cost"_a = r.initial_cost, "final_cost"_a = r.final_cost,
+                          "num_iterations"_a = r.num_iterations, "num_successful_steps"_a = r.num_successful_steps,
+                          "num_unsuccessful_steps"_a = r.num_unsuccessful_steps, "termination_type"_a = r.termination_type,
+                          "block_evaluations"_a = r.block_evaluations));
+    }
+    return py::dict("results"_a = out, "n_waves"_a = n_waves, "h2d_bytes"_a = s.h2d_bytes, "solve_time_s"_a = s.solve_time_s,
+                    "total_time_s"_a = s.total_time_s);
+  }, "ctx"_a, "problem"_a, "interpolation"_a = py::dict(), "options"_a = py::dict());
   m.def("refs_compute", [](Context& ctx, py::dict problem, py::dict interpolation, int loss_type, double loss_scale, int iters) {
     Fields f{problem, {}};
     pxr_ba_desc d = ba_desc(f);

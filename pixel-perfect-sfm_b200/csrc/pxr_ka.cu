@@ -21,6 +21,7 @@
 
 #include "pxr_fm_eval.cuh"
 #include "pxr_internal.h"
+#include "pxr_lm.cuh"
 
 namespace pxr {
 
@@ -427,10 +428,9 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
   }
   __syncthreads();
   int iter = 0, invalid = 0, n_succ = 0, n_unsucc = 0, term = 1;
-  // ceres TrustRegionStepEvaluator (uniform over the CTA: every input is a block-wide reduction); max_nonmonotonic == 0
-  // reproduces the monotonic rule  rel = (current_cost - candidate_cost) / mcc  bit for bit
-  double ev_min = x_cost, ev_ref = x_cost, ev_cand = x_cost, ev_acc_ref = 0.0, ev_acc_cand = 0.0;
-  int ev_nonmono = 0;
+  // ceres TrustRegionStepEvaluator (uniform over the CTA: every input is a block-wide reduction)
+  DevStepEvaluator ev;
+  ev.init(x_cost, a.max_nonmonotonic);
   double minimum_cost = x_cost;     // ceres keeps the lowest-cost iterate in the user's parameter blocks
   while (true) {
     // FinalizeIterationAndCheckIfMinimizerCanContinue
@@ -564,9 +564,7 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
     double sn = 0; { double v = 0; for (int i = tid; i < n; i += kKAThreads) { const double d = w.x[i] - w.cand[i]; v += d * d; } sn = sqrt(block_sum(v)); }
     if (sn <= a.ptol * (w.ctrl[C_XNORM] + a.ptol)) { term = 0; break; }            // parameter tolerance: step not applied
     if (fabs(x_cost - candidate_cost) <= a.ftol * x_cost) { term = 0; break; }     // function tolerance: step not applied
-    double rel = (w.ctrl[C_CURCOST] - candidate_cost) / mcc;
-    if (candidate_cost >= 1.7976931348623157e308) rel = -1.7976931348623157e308;
-    else if (a.max_nonmonotonic > 0) rel = fmax(rel, (ev_ref - candidate_cost) / (ev_acc_ref + mcc));
+    const double rel = ev.quality(candidate_cost, mcc);
     if (rel > a.min_rel_dec) {
       __syncthreads();
       for (int i = tid; i < n; i += kKAThreads) w.x[i] = w.cand[i];
@@ -577,18 +575,13 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
         w.ctrl[C_GMAX] = w.ctrl[C_TMP];
         double r2 = w.ctrl[C_RADIUS] / fmax(1.0 / 3.0, 1.0 - pow(2.0 * rel - 1.0, 3.0));
         w.ctrl[C_RADIUS] = fmin(a.max_radius, r2);
-        w.ctrl[C_DECF] = 2.0; w.ctrl[C_CURCOST] = candidate_cost; w.ctrl[C_XCOST] = x_cost;
+        w.ctrl[C_DECF] = 2.0; w.ctrl[C_XCOST] = x_cost;
       }
       ++n_succ;
-      if (a.max_nonmonotonic > 0) {
-        ev_acc_cand += mcc; ev_acc_ref += mcc;
-        if (candidate_cost < ev_min) { ev_min = candidate_cost; ev_nonmono = 0; ev_cand = candidate_cost; ev_acc_cand = 0.0; }
-        else { ++ev_nonmono; if (candidate_cost > ev_cand) { ev_cand = candidate_cost; ev_acc_cand = 0.0; } }
-        if (ev_nonmono == a.max_nonmonotonic) { ev_ref = ev_cand; ev_acc_ref = ev_acc_cand; }
-        if (x_cost < minimum_cost) {    // new best iterate: it goes to the output right away
-          minimum_cost = x_cost;
-          for (int i = tid; i < n; i += kKAThreads) a.keypoints[2 * a.var_kp[vb + i / 2] + (i & 1)] = w.x[i];
-        }
+      ev.accepted(candidate_cost, mcc);
+      if (a.max_nonmonotonic > 0 && x_cost < minimum_cost) {    // new best iterate: it goes to the output right away
+        minimum_cost = x_cost;
+        for (int i = tid; i < n; i += kKAThreads) a.keypoints[2 * a.var_kp[vb + i / 2] + (i & 1)] = w.x[i];
       }
     } else {
       __syncthreads();

@@ -1,0 +1,849 @@
+// pxr_qba.cu — batched query bundle adjustment: many localization queries refined in one launch.
+//
+// Replaces a loop of _localization.QueryBundleOptimizer.run (reference localization/src/single_query_bundle_optimizer.h,
+// query_bundle_optimizer.h): per query one image pose (QuaternionManifold rotation + translation) and optionally some
+// intrinsics, against constant 3D points and fixed reference descriptors.  pxr_ba_run solves such a query with a whole
+// BA handle and a host-driven LM loop; here one CTA carries a query's whole solve:
+//   evaluation  per residual block world_to_pixel<true> + ToPixelCoordinates (K0's arithmetic), the clamped 4x4 tap window
+//               read from global memory, K1's bicubic pass, L2 normalisation and r = f - ref with the butterfly order of
+//               K1 (so the record (||r||^2, G^T r, G^T G) is K1's), scaled by rho' and accumulated into J^T J / J^T r
+//               per warp; the warps' partials are summed in warp order, so a query's bits never depend on its neighbours
+//   LM          BA::lm_begin / lm_iterate (pxr_ba.cu) for one free image, no free points, no inner iterations: Jacobi
+//               scaling from iteration zero, clamped LM diagonal, invalid steps, parameter / function / gradient
+//               tolerances, ceres' step evaluator (pxr_lm.cuh) with use_nonmonotonic_steps and the lowest-cost iterate
+//               written back, the radius update and the termination types of lm_finalize
+//   solve       exact dense Cholesky of the damped n x n system (n = 6 + free intrinsics <= 18), one thread
+// The host packs consecutive queries into waves that fit a byte budget; one wave is one launch, and the next wave's
+// upload is enqueued before the host waits for the current one.
+#include <algorithm>
+#include <chrono>
+#include <cmath>
+#include <cstdlib>
+#include <cstring>
+#include <vector>
+
+#include "pxr_fm_eval.cuh"
+#include "pxr_internal.h"
+#include "pxr_lm.cuh"
+
+namespace pxr {
+
+int fm_supported(int dtype, int C);
+
+constexpr int kQThreads = 256;
+constexpr int kQWarps = kQThreads / 32;
+constexpr int kQMaxN = 6 + kMaxK;                       // tangent columns of one query
+constexpr int kQTri = kQMaxN * (kQMaxN + 1) / 2;
+constexpr int kQPart = kQTri + kQMaxN + 1;              // one warp's partial: J^T J (lower), J^T r, cost
+constexpr int kQParams = kMaxK + 7;                     // cam params | qvec | tvec
+constexpr int kQEntries = (kQTri + kQMaxN + 31) / 32;   // J^T J / J^T r entries per lane
+
+struct QBAArgs {
+  int n_queries;
+  const int64_t* obs_begin;            // [nq+1] wave-local
+  const int32_t* cam_model; const uint32_t* cam_mask;
+  double* params;                      // [nq][kQParams] in/out
+  const uint64_t* patch;               // [nq] address of the query's patch block
+  const int64_t* patch_first;          // [nq] the query's first row of corner / scale
+  const double* xyz; const int64_t* obs_patch; const double* refs;
+  const int32_t* corner; const double* scale; double ups; int ph, pw;
+  LossParams loss; int l2_normalize;
+  int max_iter, max_invalid, max_nonmonotonic, jacobi_scaling;
+  double ftol, gtol, ptol, min_rel_dec, radius0, max_radius, min_radius, min_diag, max_diag;
+  int row_stride;                      // doubles per projected-block row in shared memory
+  pxr_qba_result* results;             // [nq]
+  pxr_iteration_summary* iters; int iter_cap;   // [nq][iter_cap] or null
+  int linearize_only;                  // pxr_qba_debug_linearize: evaluate once and report
+  double* dbg_cost; double* dbg_H; double* dbg_g; double* dbg_xy; double* dbg_rec;
+};
+
+__device__ __forceinline__ int qtri(int i, int j) { return i * (i + 1) / 2 + j; }   // i >= j
+
+// Linearisation of one query at prm (whole CTA): H (packed lower) and g in the query's tangent columns; returns the cost.
+// Each warp takes batches of 32 blocks: every lane projects one block into its shared row [u, v, x, y, Ju(n), Jv(n)],
+// then the warp evaluates the batch one block at a time, one channel group per lane.
+template <typename T, int C, bool FS>
+__device__ double qba_evaluate(const QBAArgs& a, int q, const double* prm, int model, uint32_t mask, int n, double* H,
+                               double* g, double* rows, double* part, int64_t ob, int64_t oe) {
+  constexpr int CPL = C >= 32 ? C / 32 : 1;
+  constexpr int ACTIVE = C / CPL;
+  constexpr int TAP_BYTES = C * (int)sizeof(T);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const bool active = lane < ACTIVE;
+  const int RS = a.row_stride;
+  double* wrow = rows + (size_t)warp * 32 * RS;
+  const int ntri = n * (n + 1) / 2, nent = ntri + n;
+  int ea[kQEntries], eb[kQEntries];    // this lane's entries k = lane + 32 i: H(ea, eb), or g(ea) when eb < 0
+#pragma unroll
+  for (int i = 0; i < kQEntries; ++i) {
+    const int k = lane + 32 * i;
+    ea[i] = -1; eb[i] = -1;
+    if (k < ntri) { int r = 0; while ((r + 1) * (r + 2) / 2 <= k) ++r; ea[i] = r; eb[i] = k - r * (r + 1) / 2; }
+    else if (k < nent) ea[i] = k - ntri;
+  }
+  double acc[kQEntries];
+#pragma unroll
+  for (int i = 0; i < kQEntries; ++i) acc[i] = 0.0;
+  double cost = 0.0;
+  const int Kc = cam_num_params(model);
+  const uint8_t* pbase = reinterpret_cast<const uint8_t*>(a.patch[q]);
+  const int64_t patch_bytes = (int64_t)a.ph * a.pw * TAP_BYTES;
+  const int64_t pf = a.patch_first[q];
+  for (int64_t b0 = ob + (int64_t)warp * 32; b0 < oe; b0 += kQWarps * 32) {
+    __syncwarp();
+    const int64_t o = b0 + lane;
+    if (o < oe) {
+      double X[3], xy[2], Jpose[2][6], Jpt[2][3], Jk[2][kMaxK];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) X[k] = a.xyz[3 * o + k];
+      world_to_pixel<true>(model, prm, prm + kMaxK, prm + kMaxK + 4, X, xy, Jpose, Jpt, Jk);
+      const int64_t pi = pf + a.obs_patch[o];
+      const double sx = a.scale[2 * pi], sy = a.scale[2 * pi + 1];
+      const double cx = (double)a.corner[2 * pi], cy = (double)a.corner[2 * pi + 1];
+      double* r = wrow + lane * RS;
+      r[0] = (xy[0] * sx - 0.5 - cx) * a.ups;
+      r[1] = (xy[1] * sy - 0.5 - cy) * a.ups;
+      r[2] = xy[0]; r[3] = xy[1];
+      const double s0 = sx * a.ups, s1 = sy * a.ups;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) { r[4 + k] = s0 * Jpose[0][k]; r[4 + n + k] = s1 * Jpose[1][k]; }
+      int c = 6;
+#pragma unroll
+      for (int k = 0; k < kMaxK; ++k)
+        if (k < Kc && !((mask >> k) & 1u)) { r[4 + c] = s0 * Jk[0][k]; r[4 + n + c] = s1 * Jk[1][k]; ++c; }
+    }
+    __syncwarp();
+    const int nb = (int)min((int64_t)32, oe - b0);
+    for (int j = 0; j < nb; ++j) {
+      const double* r = wrow + j * RS;
+      const int64_t oj = b0 + j;
+      const double u = r[0], v = r[1];
+      const double fu = floor(u), fv = floor(v);
+      const int col = (int)fmin(fmax(fu, -4.0), (double)a.pw + 4.0);   // as K1: NaN / far projections clamp to the border
+      const int row = (int)fmin(fmax(fv, -4.0), (double)a.ph + 4.0);
+      const uint8_t* src = pbase + a.obs_patch[oj] * patch_bytes;
+      GlobalWindow w;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        w.rowp[i] = src + (int64_t)min(max(row - 1 + i, 0), a.ph - 1) * a.pw * TAP_BYTES;
+        w.coff[i] = min(max(col - 1 + i, 0), a.pw - 1) * TAP_BYTES;
+      }
+      double f[CPL], fr[CPL], fc[CPL], res[CPL], red[6];
+#pragma unroll
+      for (int k = 0; k < CPL; ++k) { f[k] = 0.0; fr[k] = 0.0; fc[k] = 0.0; res[k] = 0.0; }
+      if (active) bicubic_window<T, C, CPL, true, FS>(w, lane, u - fu, v - fv, f, fr, fc);
+      normalize_and_reduce<CPL, true, true>(active, a.l2_normalize != 0, a.refs + oj * C + lane * CPL, f, fr, fc, res, red,
+                                            lane);
+      double rho[3];
+      loss_eval(a.loss, 1.0, red[0], rho);
+      cost += 0.5 * rho[0];
+      const double bu = rho[1] * red[1], bv = rho[1] * red[2];
+      const double auu = rho[1] * red[3], auv = rho[1] * red[4], avv = rho[1] * red[5];
+      const double* Ju = r + 4;
+      const double* Jv = r + 4 + n;
+#pragma unroll
+      for (int i = 0; i < kQEntries; ++i) {
+        const int ia = ea[i], ib = eb[i];
+        if (ia < 0) continue;
+        if (ib >= 0) {      // ba_build_kernel's camera block term
+          const double aju = auu * Ju[ia] + auv * Jv[ia], ajv = auv * Ju[ia] + avv * Jv[ia];
+          acc[i] += Ju[ib] * aju + Jv[ib] * ajv;
+        } else {
+          acc[i] += Ju[ia] * bu + Jv[ia] * bv;
+        }
+      }
+      if (a.linearize_only && lane == 0) {
+        if (a.dbg_rec) {
+          double* rec = a.dbg_rec + oj * 8;
+          for (int k = 0; k < 6; ++k) rec[k] = red[k];
+          rec[6] = 0.0; rec[7] = 0.0;
+        }
+        if (a.dbg_xy) { a.dbg_xy[2 * oj] = r[2]; a.dbg_xy[2 * oj + 1] = r[3]; }
+      }
+    }
+  }
+  double* mine = part + warp * kQPart;
+#pragma unroll
+  for (int i = 0; i < kQEntries; ++i)
+    if (ea[i] >= 0) mine[lane + 32 * i] = acc[i];
+  if (lane == 0) mine[nent] = cost;
+  __syncthreads();
+  for (int k = threadIdx.x; k <= nent; k += kQThreads) {   // fixed order over the warps
+    double s = 0.0;
+    for (int wi = 0; wi < kQWarps; ++wi) s += part[wi * kQPart + k];
+    if (k < ntri) H[k] = s;
+    else if (k < nent) g[k - ntri] = s;
+    else part[kQWarps * kQPart] = s;
+  }
+  __syncthreads();
+  const double total = part[kQWarps * kQPart];
+  __syncthreads();
+  return total;
+}
+
+// ceres' gradient_max_norm = || x - Plus(x, -g) ||_inf, as ba_gradmax_kernel forms it for one image and its camera
+__device__ double qba_gradmax(const double* g, const double* qv, int n) {
+  const double ng[3] = {-g[0], -g[1], -g[2]};
+  double qn[4];
+  quaternion_plus(qv, ng, qn);
+  double m = 0.0;
+  for (int k = 0; k < 4; ++k) m = fmax(m, fabs(qv[k] - qn[k]));
+  for (int k = 3; k < n; ++k) m = fmax(m, fabs(g[k]));
+  return m;
+}
+
+enum { QA_STOP = 0, QA_SKIP = 1, QA_EVAL = 2 };
+
+template <typename T, int C, bool FS>
+__global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
+  extern __shared__ __align__(16) double qrows[];
+  __shared__ double sH[2][kQTri], sg[2][kQMaxN], sx[3][kQParams];   // parameters: 0 current, 1 candidate, 2 best
+  __shared__ double spart[kQWarps * kQPart + 1];
+  __shared__ int sctl[2];                                           // action, current linearisation set
+  const int q = blockIdx.x, tid = threadIdx.x;
+  if (q >= a.n_queries) return;
+  const int64_t ob = a.obs_begin[q], oe = a.obs_begin[q + 1];
+  pxr_qba_result* res = a.results + q;
+  auto report = [&](int status, double c0, double c1, int term, int64_t evals) {
+    res->status = status; res->num_residual_blocks = (int32_t)(oe - ob);
+    res->initial_cost = c0; res->final_cost = c1; res->num_iterations = 0;
+    res->num_successful_steps = 0; res->num_unsuccessful_steps = 0; res->termination_type = term;
+    res->block_evaluations = evals;
+  };
+  if (oe <= ob) {      // not solved (QueryBundleOptimizer::SolveProblem returns false): parameters untouched
+    if (tid == 0) report(PXR_OK, 0.0, 0.0, 1, 0);
+    return;
+  }
+  const int model = a.cam_model[q];
+  const int Kc = cam_num_params(model);
+  const uint32_t mask = a.cam_mask[q];
+  int n = 6;
+  for (int k = 0; k < Kc; ++k) n += ((mask >> k) & 1u) ? 0 : 1;
+  for (int i = tid; i < kQParams; i += kQThreads) sx[0][i] = a.params[(int64_t)q * kQParams + i];
+  __syncthreads();
+  double x_cost = qba_evaluate<T, C, FS>(a, q, sx[0], model, mask, n, sH[0], sg[0], qrows, spart, ob, oe);
+  int64_t evals = oe - ob;
+  if (a.linearize_only) {
+    const int ntri = n * (n + 1) / 2;
+    if (tid == 0 && a.dbg_cost) a.dbg_cost[q] = x_cost;
+    if (a.dbg_H)
+      for (int k = tid; k < kQMaxN * kQMaxN; k += kQThreads) {
+        const int i = k / kQMaxN, j = k % kQMaxN;
+        a.dbg_H[(int64_t)q * kQMaxN * kQMaxN + k] = (i < n && j <= i) ? sH[0][qtri(i, j)] : 0.0;
+      }
+    if (a.dbg_g)
+      for (int k = tid; k < kQMaxN; k += kQThreads) a.dbg_g[(int64_t)q * kQMaxN + k] = k < n ? sg[0][k] : 0.0;
+    (void)ntri;
+    return;
+  }
+  if (!isfinite(x_cost)) {     // BA::lm_begin: "initial cost is not finite"
+    if (tid == 0) report(PXR_ERR_NUMERIC, x_cost, x_cost, 2, evals);
+    return;
+  }
+  // ---- LM state: thread 0 takes every scalar decision, the CTA evaluates
+  __shared__ double sL[kQTri], sd[kQMaxN], sscale[kQMaxN];
+  const double initial_cost = x_cost;
+  double radius = a.radius0, decf = 2.0, min_cost = x_cost, mcc = 0.0, step_norm = 0.0, x_norm = 0.0, prev_gmax = 0.0;
+  int n_succ = 0, n_unsucc = 0, num_invalid = 0, term = 1, n_its = 0, cur = 0;
+  bool pending = true, best_is_current = true;
+  pxr_iteration_summary it = pxr_iteration_summary();
+  DevStepEvaluator ev;
+  double xn_points = 0.0;     // ||X||^2 of the constant points: part of ceres' ||x|| (ba_plus_kernel)
+  if (tid == 0) {
+    for (int i = 0; i < n; ++i) sscale[i] = a.jacobi_scaling ? 1.0 / (1.0 + sqrt(sH[0][qtri(i, i)])) : 1.0;
+    for (int64_t o = ob; o < oe; ++o)
+      for (int k = 0; k < 3; ++k) { const double x = a.xyz[3 * o + k]; xn_points += x * x; }
+    it.cost = x_cost;
+    it.gradient_max_norm = qba_gradmax(sg[0], sx[0] + kMaxK, n);
+    ev.init(x_cost, a.max_nonmonotonic);
+  }
+  while (true) {
+    if (tid == 0) {
+      int action = QA_EVAL;
+      // FinalizeIterationAndCheckIfMinimizerCanContinue (BA::lm_finalize)
+      if (pending) {
+        if (it.step_is_successful) { ++n_succ; if (x_cost < min_cost) min_cost = x_cost; }
+        else if (it.iteration > 0) ++n_unsucc;
+        it.trust_region_radius = radius;
+        if (a.iters && n_its < a.iter_cap) a.iters[(int64_t)q * a.iter_cap + n_its] = it;
+        ++n_its;
+        pending = false;
+      }
+      if (it.iteration >= a.max_iter) { term = 1; action = QA_STOP; }
+      else if (it.gradient_max_norm <= a.gtol) { term = 0; action = QA_STOP; }
+      else if (radius < a.min_radius) { term = 0; action = QA_STOP; }
+      if (action != QA_STOP) {
+        prev_gmax = it.gradient_max_norm;
+        const int iteration = it.iteration + 1;
+        it = pxr_iteration_summary();
+        it.iteration = iteration;
+        pending = true;
+        // ---- LM step: (H + D) delta = -g, D = clamp(diag(H) s^2, lo, hi) / (radius s^2)   (ba_d2_kernel)
+        const double* H = sH[cur];
+        const double* g = sg[cur];
+        double* L = sL;
+        double* d = sd;
+        for (int i = 0; i < n * (n + 1) / 2; ++i) L[i] = H[i];
+        for (int i = 0; i < n; ++i) {
+          const double s2 = sscale[i] * sscale[i];
+          L[qtri(i, i)] += fmin(fmax(H[qtri(i, i)] * s2, a.min_diag), a.max_diag) / (radius * s2);
+        }
+        bool ok = true;
+        for (int j = 0; j < n && ok; ++j) {
+          double djj = L[qtri(j, j)];
+          for (int k = 0; k < j; ++k) djj -= L[qtri(j, k)] * L[qtri(j, k)];
+          if (!(djj > 0.0) || !isfinite(djj)) { ok = false; break; }
+          const double ljj = sqrt(djj);
+          L[qtri(j, j)] = ljj;
+          for (int i = j + 1; i < n; ++i) {
+            double v = L[qtri(i, j)];
+            for (int k = 0; k < j; ++k) v -= L[qtri(i, k)] * L[qtri(j, k)];
+            L[qtri(i, j)] = v / ljj;
+          }
+        }
+        double acc = 0.0;
+        if (ok) {
+          for (int i = 0; i < n; ++i) {
+            double v = -g[i];
+            for (int k = 0; k < i; ++k) v -= L[qtri(i, k)] * d[k];
+            d[i] = v / L[qtri(i, i)];
+          }
+          for (int i = n - 1; i >= 0; --i) {
+            double v = d[i];
+            for (int k = i + 1; k < n; ++k) v -= L[qtri(k, i)] * d[k];
+            d[i] = v / L[qtri(i, i)];
+          }
+          // model cost change = -(g.d + d^T H d / 2): ba_model_cost_kernel's sum over the blocks, in closed form
+          for (int i = 0; i < n; ++i) {
+            double hd = 0.0;
+            for (int j = 0; j < n; ++j) hd += (i >= j ? H[qtri(i, j)] : H[qtri(j, i)]) * d[j];
+            acc += g[i] * d[i] + 0.5 * d[i] * hd;
+          }
+        }
+        mcc = -acc;
+        const bool valid = ok && isfinite(acc) && mcc > 0.0;
+        it.linear_solver_iterations = 1;
+        it.step_is_valid = valid;
+        if (!valid) {
+          if (++num_invalid >= a.max_invalid) { term = 2; action = QA_STOP; }
+          else {
+            radius /= decf; decf *= 2.0;
+            it.cost = x_cost; it.gradient_max_norm = prev_gmax;
+            action = QA_SKIP;
+          }
+        } else {
+          num_invalid = 0;
+          // ---- candidate = Plus(x, delta) and the norms ba_plus_kernel forms (this image and its camera)
+          const double* x = sx[0];
+          double* xc = sx[1];
+          const double* qv = x + kMaxK;
+          const double* tv = x + kMaxK + 4;
+          double qn[4], dnc = 0.0, xnc = 0.0;
+          quaternion_plus(qv, d, qn);
+          for (int k = 0; k < 3; ++k) { const double tp = tv[k] + d[3 + k]; xc[kMaxK + 4 + k] = tp; dnc += (tp - tv[k]) * (tp - tv[k]); }
+          for (int k = 0; k < 4; ++k) { xc[kMaxK + k] = qn[k]; dnc += (qn[k] - qv[k]) * (qn[k] - qv[k]); xnc += qv[k] * qv[k]; }
+          for (int k = 0; k < 3; ++k) xnc += tv[k] * tv[k];
+          int la = 6;
+          for (int k = 0; k < kMaxK; ++k) {
+            const double c0 = x[k];
+            double cpv = c0;
+            if (k < Kc && !((mask >> k) & 1u)) cpv += d[la++];
+            xc[k] = cpv;
+            dnc += (cpv - c0) * (cpv - c0);
+            if (k < Kc) xnc += c0 * c0;
+          }
+          step_norm = sqrt(dnc);
+          x_norm = sqrt(xn_points + xnc);
+        }
+      }
+      sctl[0] = action; sctl[1] = cur;
+    }
+    __syncthreads();
+    const int action = sctl[0], set = sctl[1];
+    __syncthreads();
+    if (action == QA_STOP) break;
+    if (action == QA_SKIP) continue;
+    // trial point, evaluated with the Jacobian: when accepted it is the next linearisation (BA's speculative pass)
+    double candidate_cost = qba_evaluate<T, C, FS>(a, q, sx[1], model, mask, n, sH[1 - set], sg[1 - set], qrows, spart, ob, oe);
+    evals += oe - ob;
+    if (tid == 0) {
+      int act = QA_EVAL;
+      if (!isfinite(candidate_cost)) candidate_cost = 1.7976931348623157e308;
+      it.step_norm = step_norm;
+      if (step_norm <= a.ptol * (x_norm + a.ptol)) { term = 0; act = QA_STOP; }    // parameter tolerance: step not applied
+      else {
+        it.cost_change = x_cost - candidate_cost;
+        if (fabs(it.cost_change) <= a.ftol * x_cost) { term = 0; act = QA_STOP; }  // function tolerance: step not applied
+        else {
+          it.relative_decrease = ev.quality(candidate_cost, mcc);
+          if (it.relative_decrease > a.min_rel_dec) {
+            if (a.max_nonmonotonic > 0 && !(candidate_cost < min_cost) && best_is_current) {
+              for (int i = 0; i < kQParams; ++i) sx[2][i] = sx[0][i];    // leaving the best iterate: keep it
+              best_is_current = false;
+            } else if (a.max_nonmonotonic > 0 && candidate_cost < min_cost) {
+              best_is_current = true;
+            }
+            for (int i = 0; i < kQParams; ++i) sx[0][i] = sx[1][i];
+            cur = 1 - cur;
+            x_cost = candidate_cost;
+            it.cost = x_cost;
+            it.gradient_max_norm = qba_gradmax(sg[cur], sx[0] + kMaxK, n);
+            it.step_is_successful = 1;
+            radius = radius / fmax(1.0 / 3.0, 1.0 - pow(2.0 * it.relative_decrease - 1.0, 3.0));
+            radius = fmin(a.max_radius, radius);
+            decf = 2.0;
+            ev.accepted(candidate_cost, mcc);
+          } else {
+            it.step_is_successful = 0;
+            it.cost = candidate_cost;
+            it.gradient_max_norm = prev_gmax;
+            radius /= decf; decf *= 2.0;
+          }
+        }
+      }
+      sctl[0] = act;
+    }
+    __syncthreads();
+    const int act = sctl[0];
+    __syncthreads();
+    if (act == QA_STOP) break;
+  }
+  if (tid == 0) {
+    if (x_cost < min_cost) min_cost = x_cost;
+    const double* out = (a.max_nonmonotonic > 0 && !best_is_current) ? sx[2] : sx[0];
+    for (int i = 0; i < kQParams; ++i) a.params[(int64_t)q * kQParams + i] = out[i];
+    res->status = PXR_OK;
+    res->num_residual_blocks = (int32_t)(oe - ob);
+    res->initial_cost = initial_cost;
+    res->final_cost = min_cost;
+    res->num_iterations = n_its;
+    res->num_successful_steps = n_succ;
+    res->num_unsuccessful_steps = n_unsucc;
+    res->termination_type = term;
+    res->block_evaluations = evals;
+  }
+}
+
+template <typename T, int C, bool FS>
+static int launch_qba_t(pxr_ctx* ctx, const QBAArgs& a, size_t smem) {
+  PXR_CUDA(cudaFuncSetAttribute(qba_solve_kernel<T, C, FS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  PXR_LAUNCH(ctx, (qba_solve_kernel<T, C, FS>), a.n_queries, kQThreads, smem, a);
+  PXR_CUDA(cudaGetLastError());
+  return PXR_OK;
+}
+
+static int launch_qba(pxr_ctx* ctx, int dtype, int C, bool fs, const QBAArgs& a, size_t smem) {
+#define PXR_QBA_CASE(T, CC) \
+  if (C == CC) return fs ? launch_qba_t<T, CC, true>(ctx, a, smem) : launch_qba_t<T, CC, false>(ctx, a, smem);
+  if (dtype == PXR_F16) {
+    PXR_QBA_CASE(__half, 128) PXR_QBA_CASE(__half, 64) PXR_QBA_CASE(__half, 32) PXR_QBA_CASE(__half, 16)
+    PXR_QBA_CASE(__half, 8) PXR_QBA_CASE(__half, 256)
+  } else if (dtype == PXR_F32) {
+    PXR_QBA_CASE(float, 128) PXR_QBA_CASE(float, 64) PXR_QBA_CASE(float, 16)
+  } else if (dtype == PXR_F64) {
+    PXR_QBA_CASE(double, 128) PXR_QBA_CASE(double, 16)
+  }
+#undef PXR_QBA_CASE
+  return fail(PXR_ERR_UNSUPPORTED, "Unsupported dimensions (CHANNELS,N_NODES).");
+}
+
+// ---- host side --------------------------------------------------------------------------------------------------
+constexpr double kQueryStateBytes = kQParams * 8 + 8 + 8 + 8 + 4 + 4;   // params, obs_begin, patch address, first row, model, mask
+
+static size_t dtype_bytes(int dt) { return dt == PXR_F16 ? 2 : (dt == PXR_F32 ? 4 : 8); }
+
+static bool on_device(const void* p) {
+  cudaPointerAttributes pa;
+  if (!p || cudaPointerGetAttributes(&pa, p) != cudaSuccess) { cudaGetLastError(); return false; }
+  return pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged;
+}
+
+static int check_qba(const pxr_qba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so) {
+  if (!d) return fail(PXR_ERR_INVALID_ARGUMENT, "desc is NULL");
+  if (d->n_queries < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "n_queries < 0");
+  if (d->n_queries > 0 && (!d->cam_model || !d->cam_params || !d->cam_const_mask || !d->qvec || !d->tvec ||
+                           !d->obs_begin || !d->patch_blocks || !d->patch_counts))
+    return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  if (so && so->use_inner_iterations)
+    return fail(PXR_ERR_INVALID_ARGUMENT, "query bundle adjustment has no free points: use_inner_iterations must be 0");
+  if (so && so->linear_solver == PXR_SOLVER_ITERATIVE_SCHUR)
+    return fail(PXR_ERR_UNSUPPORTED, "ITERATIVE_SCHUR is not supported for query bundle adjustment (exact dense solve)");
+  if (ic && ic->check_bounds) return fail(PXR_ERR_UNSUPPORTED, "check_bounds=true is not supported on this path");
+  if (d->channels < 8 || !fm_supported(d->patch_dtype, d->channels))
+    return fail(PXR_ERR_UNSUPPORTED, "Unsupported dimensions (CHANNELS,N_NODES).");
+  if (d->ph < 1 || d->pw < 1) return fail(PXR_ERR_INVALID_ARGUMENT, "bad patch size");
+  if (!(d->upsampling_factor > 0.0)) return fail(PXR_ERR_INVALID_ARGUMENT, "upsampling_factor must be > 0");
+  if (d->n_queries == 0) return PXR_OK;
+  if (d->obs_begin[0] != 0) return fail(PXR_ERR_INVALID_ARGUMENT, "obs_begin[0] must be 0");
+  int64_t n_patches = 0;
+  for (int q = 0; q < d->n_queries; ++q) {
+    if (d->obs_begin[q + 1] < d->obs_begin[q]) return fail(PXR_ERR_INVALID_ARGUMENT, "obs_begin must be non-decreasing");
+    if (cam_num_params(d->cam_model[q]) == 0) return fail(PXR_ERR_UNSUPPORTED, "unsupported camera model id %d", d->cam_model[q]);
+    if (d->patch_counts[q] < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "patch_counts[%d] < 0", q);
+    if (d->patch_counts[q] > 0 && !d->patch_blocks[q]) return fail(PXR_ERR_INVALID_ARGUMENT, "patch block %d is NULL", q);
+    n_patches += d->patch_counts[q];
+  }
+  const int64_t n_obs = d->obs_begin[d->n_queries];
+  if (n_obs > 0 && (!d->xyz || !d->obs_patch || !d->refs)) return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  if (n_patches > 0 && (!d->corner || !d->scale)) return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  for (int q = 0; q < d->n_queries; ++q)
+    for (int64_t o = d->obs_begin[q]; o < d->obs_begin[q + 1]; ++o)
+      if (d->obs_patch[o] < 0 || d->obs_patch[o] >= d->patch_counts[q])
+        return fail(PXR_ERR_INVALID_ARGUMENT, "obs_patch[%lld] is not a patch of query %d", (long long)o, q);
+  return PXR_OK;
+}
+
+static int qba_args(pxr_ctx* ctx, const pxr_qba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so) {
+  PXR_TRY(check_qba(d, ic, so));
+  if (ctx) return PXR_OK;
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
+    cudaGetLastError();
+    return fail(PXR_ERR_NO_DEVICE, "no CUDA device available; libpxr has no CPU fallback");
+  }
+  return fail(PXR_ERR_INVALID_ARGUMENT, "ctx is NULL");
+}
+
+struct WavePlan {
+  std::vector<int32_t> begin;       // [n_waves + 1]
+  std::vector<double> bytes;        // [n_waves]
+  std::vector<uint8_t> host_patch;  // [n_queries] 1: the block is uploaded
+};
+
+static double query_bytes(const pxr_qba_desc* d, int q, bool host_patch) {
+  const double patch = (double)d->ph * d->pw * d->channels * dtype_bytes(d->patch_dtype);
+  const double m = (double)(d->obs_begin[q + 1] - d->obs_begin[q]);
+  return (host_patch ? d->patch_counts[q] * patch : 0.0) + m * (d->channels * 8.0 + 24.0 + 8.0) +
+         d->patch_counts[q] * 16.0 + kQueryStateBytes;
+}
+
+// consecutive queries while the wave fits the budget; a query larger than the budget gets a wave of its own
+static void plan_waves(const pxr_qba_desc* d, double budget, WavePlan* p) {
+  p->begin.assign(1, 0); p->bytes.clear();
+  p->host_patch.assign((size_t)d->n_queries, 0);
+  double cur = 8.0;      // obs_begin's closing entry
+  for (int q = 0; q < d->n_queries; ++q) {
+    p->host_patch[q] = (d->patch_counts[q] > 0 && !on_device(d->patch_blocks[q])) ? 1 : 0;
+    const double b = query_bytes(d, q, p->host_patch[q] != 0);
+    if (q > p->begin.back() && cur + b > budget) { p->bytes.push_back(cur); p->begin.push_back(q); cur = 8.0; }
+    cur += b;
+  }
+  if (d->n_queries > 0) { p->bytes.push_back(cur); p->begin.push_back(d->n_queries); }
+}
+
+static int wave_budget(const pxr_qba_desc* d, double* budget) {
+  if (d->max_wave_bytes > 0.0) { *budget = d->max_wave_bytes; return PXR_OK; }
+  int count = 0;
+  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
+    cudaGetLastError();
+    return fail(PXR_ERR_NO_DEVICE, "max_wave_bytes 0 means half of the free device memory, and there is no CUDA device");
+  }
+  size_t fr = 0, tot = 0;
+  PXR_CUDA(cudaMemGetInfo(&fr, &tot));
+  *budget = 0.5 * (double)fr;
+  return PXR_OK;
+}
+
+// Device memory of one wave: [host patch blocks | refs | xyz | obs_patch | corner | scale | per-query state]
+struct WaveBufs {
+  DevBuf<uint8_t> arena;
+  DevBuf<pxr_qba_result> results;
+  DevBuf<pxr_iteration_summary> iters;
+  std::vector<uint8_t> state;       // host staging of the per-query state
+};
+struct WaveView {
+  int q0, nq; int64_t o0, no, p0, np;
+  size_t off_refs, off_xyz, off_op, off_corner, off_scale, off_params, off_ob, off_ptr, off_pf, off_model, off_mask, end;
+};
+
+static WaveView wave_view(const pxr_qba_desc* d, const WavePlan& p, int w) {
+  WaveView v;
+  v.q0 = p.begin[w]; v.nq = p.begin[w + 1] - v.q0;
+  v.o0 = d->obs_begin[v.q0]; v.no = d->obs_begin[v.q0 + v.nq] - v.o0;
+  v.p0 = 0; for (int q = 0; q < v.q0; ++q) v.p0 += d->patch_counts[q];
+  v.np = 0; for (int q = v.q0; q < v.q0 + v.nq; ++q) v.np += d->patch_counts[q];
+  const size_t patch = (size_t)d->ph * d->pw * d->channels * dtype_bytes(d->patch_dtype);
+  size_t off = 0;
+  for (int q = v.q0; q < v.q0 + v.nq; ++q) if (p.host_patch[q]) off += (size_t)d->patch_counts[q] * patch;
+  v.off_refs = off; off += (size_t)v.no * d->channels * 8;
+  v.off_xyz = off; off += (size_t)v.no * 24;
+  v.off_op = off; off += (size_t)v.no * 8;
+  v.off_corner = off; off += (size_t)v.np * 8;
+  v.off_scale = off; off += (size_t)v.np * 16;
+  v.off_params = off; off += (size_t)v.nq * kQParams * 8;
+  v.off_ob = off; off += (size_t)(v.nq + 1) * 8;
+  v.off_ptr = off; off += (size_t)v.nq * 8;
+  v.off_pf = off; off += (size_t)v.nq * 8;
+  v.off_model = off; off += (size_t)v.nq * 4;
+  v.off_mask = off; off += (size_t)v.nq * 4;
+  v.end = off;
+  return v;
+}
+
+// enqueue the upload of wave v into `b` on `stream`
+static int upload_wave(pxr_ctx* ctx, const pxr_qba_desc* d, const WavePlan& p, const WaveView& v, WaveBufs& b,
+                       cudaStream_t stream, double* h2d) {
+  uint8_t* base = b.arena.p;
+  const size_t patch = (size_t)d->ph * d->pw * d->channels * dtype_bytes(d->patch_dtype);
+  // per-query state, staged on the host
+  b.state.assign(v.end - v.off_params, 0);
+  uint8_t* st = b.state.data();
+  double* params = reinterpret_cast<double*>(st);
+  int64_t* obl = reinterpret_cast<int64_t*>(st + (v.off_ob - v.off_params));
+  uint64_t* ptrs = reinterpret_cast<uint64_t*>(st + (v.off_ptr - v.off_params));
+  int64_t* pf = reinterpret_cast<int64_t*>(st + (v.off_pf - v.off_params));
+  int32_t* model = reinterpret_cast<int32_t*>(st + (v.off_model - v.off_params));
+  uint32_t* mask = reinterpret_cast<uint32_t*>(st + (v.off_mask - v.off_params));
+  std::vector<const void*> srcs;
+  std::vector<size_t> sizes;
+  size_t slab = 0;
+  int64_t prow = 0;
+  for (int i = 0; i < v.nq; ++i) {
+    const int q = v.q0 + i;
+    std::memcpy(params + (size_t)i * kQParams, d->cam_params + (size_t)q * kMaxK, kMaxK * 8);
+    std::memcpy(params + (size_t)i * kQParams + kMaxK, d->qvec + (size_t)q * 4, 32);
+    std::memcpy(params + (size_t)i * kQParams + kMaxK + 4, d->tvec + (size_t)q * 3, 24);
+    obl[i] = d->obs_begin[q] - v.o0;
+    pf[i] = prow; prow += d->patch_counts[q];
+    model[i] = d->cam_model[q]; mask[i] = d->cam_const_mask[q];
+    if (p.host_patch[q]) {
+      ptrs[i] = (uint64_t)(base + slab);
+      srcs.push_back(d->patch_blocks[q]); sizes.push_back((size_t)d->patch_counts[q] * patch);
+      slab += sizes.back();
+    } else {
+      ptrs[i] = (uint64_t)d->patch_blocks[q];
+    }
+  }
+  obl[v.nq] = v.no;
+  auto seg = [&](const void* src, size_t bytes) { srcs.push_back(src); sizes.push_back(bytes); };
+  seg(d->refs ? d->refs + v.o0 * d->channels : nullptr, (size_t)v.no * d->channels * 8);
+  seg(d->xyz ? d->xyz + v.o0 * 3 : nullptr, (size_t)v.no * 24);
+  seg(d->obs_patch ? d->obs_patch + v.o0 : nullptr, (size_t)v.no * 8);
+  seg(d->corner ? d->corner + v.p0 * 2 : nullptr, (size_t)v.np * 8);
+  seg(d->scale ? d->scale + v.p0 * 2 : nullptr, (size_t)v.np * 16);
+  seg(st, b.state.size());
+  // segments of zero bytes (no observations) are skipped by upload_segments
+  for (size_t i = 0; i < srcs.size(); ++i) if (!sizes[i]) srcs[i] = st;
+  PXR_TRY(upload_segments(ctx, base, srcs.data(), sizes.data(), (int)srcs.size(), h2d, stream));
+  return PXR_OK;
+}
+
+static QBAArgs make_args(const pxr_qba_desc* d, const pxr_interp_config& ic, const pxr_solver_options& so,
+                         const WaveView& v, WaveBufs& b, int iter_cap) {
+  uint8_t* base = b.arena.p;
+  QBAArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.n_queries = v.nq;
+  a.obs_begin = reinterpret_cast<const int64_t*>(base + v.off_ob);
+  a.cam_model = reinterpret_cast<const int32_t*>(base + v.off_model);
+  a.cam_mask = reinterpret_cast<const uint32_t*>(base + v.off_mask);
+  a.params = reinterpret_cast<double*>(base + v.off_params);
+  a.patch = reinterpret_cast<const uint64_t*>(base + v.off_ptr);
+  a.patch_first = reinterpret_cast<const int64_t*>(base + v.off_pf);
+  a.xyz = reinterpret_cast<const double*>(base + v.off_xyz);
+  a.obs_patch = reinterpret_cast<const int64_t*>(base + v.off_op);
+  a.refs = reinterpret_cast<const double*>(base + v.off_refs);
+  a.corner = reinterpret_cast<const int32_t*>(base + v.off_corner);
+  a.scale = reinterpret_cast<const double*>(base + v.off_scale);
+  a.ups = d->upsampling_factor; a.ph = d->ph; a.pw = d->pw;
+  a.loss.type = so.loss_type; a.loss.a = so.loss_scale; a.l2_normalize = ic.l2_normalize;
+  a.max_iter = so.max_num_iterations; a.max_invalid = so.max_num_consecutive_invalid_steps;
+  a.max_nonmonotonic = so.use_nonmonotonic_steps ? so.max_consecutive_nonmonotonic_steps : 0;
+  a.jacobi_scaling = so.jacobi_scaling;
+  a.ftol = so.function_tolerance; a.gtol = so.gradient_tolerance; a.ptol = so.parameter_tolerance;
+  a.min_rel_dec = so.min_relative_decrease; a.radius0 = so.initial_trust_region_radius;
+  a.max_radius = so.max_trust_region_radius; a.min_radius = so.min_trust_region_radius;
+  a.min_diag = so.min_lm_diagonal; a.max_diag = so.max_lm_diagonal;
+  int nmax = 6;
+  for (int q = v.q0; q < v.q0 + v.nq; ++q) {
+    int n = 6;
+    for (int k = 0; k < cam_num_params(d->cam_model[q]); ++k) n += ((d->cam_const_mask[q] >> k) & 1u) ? 0 : 1;
+    nmax = std::max(nmax, n);
+  }
+  a.row_stride = (4 + 2 * nmax) | 1;
+  a.results = b.results.p;
+  a.iters = iter_cap > 0 ? b.iters.p : nullptr; a.iter_cap = iter_cap;
+  return a;
+}
+
+static size_t qba_smem(const QBAArgs& a) { return (size_t)kQWarps * 32 * a.row_stride * sizeof(double); }
+
+}  // namespace pxr
+
+using namespace pxr;
+
+extern "C" int pxr_qba_plan_waves(const pxr_qba_desc* d, int32_t* wave_begin, int32_t* n_waves, double* wave_bytes) {
+  PXR_TRY(check_qba(d, nullptr, nullptr));
+  if (!wave_begin || !n_waves) return fail(PXR_ERR_INVALID_ARGUMENT, "wave_begin / n_waves is NULL");
+  double budget = 0.0;
+  PXR_TRY(wave_budget(d, &budget));
+  WavePlan p;
+  plan_waves(d, budget, &p);
+  *n_waves = (int32_t)p.bytes.size();
+  for (size_t i = 0; i < p.begin.size(); ++i) wave_begin[i] = p.begin[i];
+  if (wave_bytes) for (size_t i = 0; i < p.bytes.size(); ++i) wave_bytes[i] = p.bytes[i];
+  return PXR_OK;
+}
+
+extern "C" int pxr_qba_run(pxr_ctx* ctx, const pxr_qba_desc* d, const pxr_interp_config* interp_in,
+                           const pxr_solver_options* opt_in, pxr_qba_result* results, pxr_iteration_summary* iterations,
+                           int32_t iterations_capacity, int32_t* n_waves_out, pxr_summary* total) {
+  const auto t0 = std::chrono::steady_clock::now();
+  PXR_TRY(qba_args(ctx, d, interp_in, opt_in));
+  if (!results && d->n_queries > 0) return fail(PXR_ERR_INVALID_ARGUMENT, "results is NULL");
+  if (iterations_capacity < 0 || (iterations_capacity > 0 && !iterations))
+    return fail(PXR_ERR_INVALID_ARGUMENT, "iterations is NULL or iterations_capacity < 0");
+  pxr_interp_config ic; if (interp_in) ic = *interp_in; else pxr_default_interp_config(&ic);
+  pxr_solver_options so; if (opt_in) so = *opt_in; else { pxr_default_ba_options(&so); so.use_inner_iterations = 0; }
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  cudaStream_t us = nullptr;
+  PXR_TRY(upload_stream(ctx, &us));
+  const int64_t launches0 = ctx->launches;
+  double budget = 0.0;
+  PXR_TRY(wave_budget(d, &budget));
+  WavePlan plan;
+  plan_waves(d, budget, &plan);
+  const int nw = (int)plan.bytes.size();
+  // two wave buffers (the next upload runs while the current wave solves) when both fit; PXR_QBA_WAVE_BUFFERS=1 keeps
+  // one (tests: the one-buffer ordering is otherwise reached only by waves near half the free memory)
+  size_t max_arena = 0; int max_nq = 0;
+  for (int w = 0; w < nw; ++w) {
+    const WaveView v = wave_view(d, plan, w);
+    max_arena = std::max(max_arena, v.end); max_nq = std::max(max_nq, v.nq);
+  }
+  size_t fr = 0, tot = 0;
+  PXR_CUDA(cudaMemGetInfo(&fr, &tot));
+  const char* one_buf = std::getenv("PXR_QBA_WAVE_BUFFERS");
+  const bool force_one = one_buf && std::atoi(one_buf) == 1;
+  const int nsets = (!force_one && nw > 1 && 2.0 * (double)max_arena < 0.9 * (double)fr) ? 2 : 1;
+  WaveBufs bufs[2];
+  // per buffer set, the pinned host copy of a wave's outputs: params | results | iteration summaries
+  const size_t out_params = (size_t)std::max(max_nq, 1) * kQParams * 8;
+  const size_t out_res = (size_t)std::max(max_nq, 1) * sizeof(pxr_qba_result);
+  const size_t out_bytes = out_params + out_res + (size_t)std::max(max_nq, 1) * iterations_capacity * sizeof(pxr_iteration_summary);
+  struct Pinned { void* p = nullptr; ~Pinned() { if (p) cudaFreeHost(p); } } hout[2];
+  for (int k = 0; k < nsets; ++k) {
+    PXR_TRY(bufs[k].arena.alloc(std::max<size_t>(max_arena, 16)));
+    PXR_TRY(bufs[k].results.alloc(std::max(max_nq, 1)));
+    if (iterations_capacity > 0) PXR_TRY(bufs[k].iters.alloc((size_t)std::max(max_nq, 1) * iterations_capacity));
+    PXR_CUDA(cudaMallocHost(&hout[k].p, out_bytes));
+  }
+  cudaEvent_t up_done[2] = {nullptr, nullptr}, k_done[2] = {nullptr, nullptr}, kt0 = nullptr, kt1 = nullptr;
+  struct Events { cudaEvent_t* e; int n; ~Events() { for (int i = 0; i < n; ++i) if (e[i]) cudaEventDestroy(e[i]); } };
+  cudaEvent_t all_ev[6];
+  Events guard{all_ev, 0};
+  for (cudaEvent_t* e : {&up_done[0], &up_done[1], &k_done[0], &k_done[1]}) {
+    PXR_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    all_ev[guard.n++] = *e;
+  }
+  PXR_CUDA(cudaEventCreate(&kt0)); all_ev[guard.n++] = kt0;
+  PXR_CUDA(cudaEventCreate(&kt1)); all_ev[guard.n++] = kt1;
+  double h2d = 0.0, kernel_ms = 0.0;
+  double ic0 = 0.0, fc = 0.0; int ns = 0, nu = 0;
+  if (nw > 0) PXR_TRY(upload_wave(ctx, d, plan, wave_view(d, plan, 0), bufs[0], us, &h2d));
+  for (int w = 0; w < nw; ++w) {
+    const int set = nsets == 2 ? (w & 1) : 0;
+    const WaveView v = wave_view(d, plan, w);
+    WaveBufs& b = bufs[set];
+    PXR_CUDA(cudaEventRecord(up_done[set], us));
+    PXR_CUDA(cudaStreamWaitEvent(s, up_done[set], 0));
+    const QBAArgs a = make_args(d, ic, so, v, b, iterations_capacity);
+    PXR_CUDA(cudaEventRecord(kt0, s));
+    PXR_TRY(launch_qba(ctx, d->patch_dtype, d->channels, ic.use_float_simd != 0, a, qba_smem(a)));
+    PXR_CUDA(cudaEventRecord(kt1, s));
+    // the wave's outputs leave the arena before k_done: a later upload into this arena waits for k_done
+    uint8_t* ho = static_cast<uint8_t*>(hout[set].p);
+    const double* params = reinterpret_cast<const double*>(ho);
+    const pxr_qba_result* wres = reinterpret_cast<const pxr_qba_result*>(ho + out_params);
+    const pxr_iteration_summary* wits = reinterpret_cast<const pxr_iteration_summary*>(ho + out_params + out_res);
+    PXR_CUDA(cudaMemcpyAsync(ho, a.params, (size_t)v.nq * kQParams * 8, cudaMemcpyDeviceToHost, s));
+    PXR_CUDA(cudaMemcpyAsync(ho + out_params, b.results.p, (size_t)v.nq * sizeof(pxr_qba_result), cudaMemcpyDeviceToHost, s));
+    if (iterations_capacity > 0)
+      PXR_CUDA(cudaMemcpyAsync(ho + out_params + out_res, b.iters.p,
+                               (size_t)v.nq * iterations_capacity * sizeof(pxr_iteration_summary), cudaMemcpyDeviceToHost, s));
+    PXR_CUDA(cudaEventRecord(k_done[set], s));
+    if (w + 1 < nw) {        // the next upload goes out before the host waits for this wave
+      const int nset = nsets == 2 ? 1 - set : 0;
+      if (nsets == 1) PXR_CUDA(cudaStreamWaitEvent(us, k_done[set], 0));
+      PXR_TRY(upload_wave(ctx, d, plan, wave_view(d, plan, w + 1), bufs[nset], us, &h2d));
+    }
+    PXR_CUDA(cudaEventSynchronize(k_done[set]));
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, kt0, kt1) == cudaSuccess) kernel_ms += ms;
+    for (int i = 0; i < v.nq; ++i) {
+      const int q = v.q0 + i;
+      const pxr_qba_result& r = wres[i];
+      results[q] = r;
+      if (iterations_capacity > 0) {
+        std::memcpy(iterations + (size_t)q * iterations_capacity, wits + (size_t)i * iterations_capacity,
+                    (size_t)iterations_capacity * sizeof(pxr_iteration_summary));
+      }
+      if (r.status != PXR_OK || r.num_residual_blocks == 0) continue;   // parameters untouched
+      const double* p = params + (size_t)i * kQParams;
+      std::memcpy(d->cam_params + (size_t)q * kMaxK, p, kMaxK * 8);
+      std::memcpy(d->qvec + (size_t)q * 4, p + kMaxK, 32);
+      std::memcpy(d->tvec + (size_t)q * 3, p + kMaxK + 4, 24);
+      ic0 += r.initial_cost; fc += r.final_cost; ns += r.num_successful_steps; nu += r.num_unsuccessful_steps;
+    }
+    if (w + 1 < nw && interrupt_pending()) {
+      cudaStreamSynchronize(us);
+      if (n_waves_out) *n_waves_out = w + 1;
+      return fail(PXR_ERR_INTERRUPTED, "interrupted by the host after wave %d of %d", w + 1, nw);
+    }
+  }
+  PXR_CUDA(cudaStreamSynchronize(us));
+  if (n_waves_out) *n_waves_out = nw;
+  if (total) {
+    const int cap = total->iterations_capacity;
+    pxr_iteration_summary* keep = total->iterations;
+    std::memset(total, 0, sizeof(*total));
+    total->iterations_capacity = cap; total->iterations = keep;
+    total->initial_cost = ic0; total->final_cost = fc;
+    total->num_residual_blocks = (int32_t)(d->n_queries ? d->obs_begin[d->n_queries] : 0);
+    total->num_residuals = (int64_t)total->num_residual_blocks * d->channels;
+    total->num_successful_steps = ns; total->num_unsuccessful_steps = nu;
+    total->h2d_bytes = h2d;
+    total->kernel_launches = ctx->launches - launches0;
+    total->total_time_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    total->solve_time_s = kernel_ms * 1e-3;
+    std::snprintf(total->message, sizeof(total->message), "%d queries in %d waves, solve kernels %.3f ms", d->n_queries, nw,
+                  kernel_ms);
+  }
+  return PXR_OK;
+}
+
+extern "C" int pxr_qba_debug_linearize(pxr_ctx* ctx, const pxr_qba_desc* d, const pxr_interp_config* interp_in,
+                                       const pxr_solver_options* opt_in, double* cost, double* H, double* g, double* xy,
+                                       double* rec) {
+  PXR_TRY(qba_args(ctx, d, interp_in, opt_in));
+  pxr_interp_config ic; if (interp_in) ic = *interp_in; else pxr_default_interp_config(&ic);
+  pxr_solver_options so; if (opt_in) so = *opt_in; else { pxr_default_ba_options(&so); so.use_inner_iterations = 0; }
+  if (d->n_queries == 0) return PXR_OK;
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  WavePlan plan;
+  plan_waves(d, 1e300, &plan);            // one wave
+  const WaveView v = wave_view(d, plan, 0);
+  WaveBufs b;
+  PXR_TRY(b.arena.alloc(std::max<size_t>(v.end, 16)));
+  PXR_TRY(b.results.alloc(v.nq));
+  double h2d = 0.0;
+  PXR_TRY(upload_wave(ctx, d, plan, v, b, s, &h2d));
+  const int64_t n_obs = v.no;
+  DevBuf<double> dc, dH, dg, dxy, drec;
+  PXR_TRY(dc.alloc(v.nq)); PXR_TRY(dH.alloc((size_t)v.nq * kQMaxN * kQMaxN)); PXR_TRY(dg.alloc((size_t)v.nq * kQMaxN));
+  PXR_TRY(dxy.alloc((size_t)std::max<int64_t>(n_obs, 1) * 2)); PXR_TRY(drec.alloc((size_t)std::max<int64_t>(n_obs, 1) * 8));
+  PXR_TRY(dc.zero(s)); PXR_TRY(dH.zero(s)); PXR_TRY(dg.zero(s)); PXR_TRY(dxy.zero(s)); PXR_TRY(drec.zero(s));
+  QBAArgs a = make_args(d, ic, so, v, b, 0);
+  a.linearize_only = 1;
+  a.dbg_cost = dc.p; a.dbg_H = dH.p; a.dbg_g = dg.p; a.dbg_xy = dxy.p; a.dbg_rec = drec.p;
+  PXR_TRY(launch_qba(ctx, d->patch_dtype, d->channels, ic.use_float_simd != 0, a, qba_smem(a)));
+  if (cost) PXR_CUDA(cudaMemcpyAsync(cost, dc.p, (size_t)v.nq * 8, cudaMemcpyDeviceToHost, s));
+  if (H) PXR_CUDA(cudaMemcpyAsync(H, dH.p, (size_t)v.nq * kQMaxN * kQMaxN * 8, cudaMemcpyDeviceToHost, s));
+  if (g) PXR_CUDA(cudaMemcpyAsync(g, dg.p, (size_t)v.nq * kQMaxN * 8, cudaMemcpyDeviceToHost, s));
+  if (xy && n_obs) PXR_CUDA(cudaMemcpyAsync(xy, dxy.p, (size_t)n_obs * 16, cudaMemcpyDeviceToHost, s));
+  if (rec && n_obs) PXR_CUDA(cudaMemcpyAsync(rec, drec.p, (size_t)n_obs * 64, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  return PXR_OK;
+}

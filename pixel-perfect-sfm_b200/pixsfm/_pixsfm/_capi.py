@@ -135,6 +135,91 @@ class KADesc(C.Structure):
                 ("ref_desc", C.c_void_p), ("n_ref_desc", C.c_int64)]
 
 
+class QBADesc(C.Structure):            # pxr_qba_desc
+    _fields_ = [("n_queries", C.c_int32), ("cam_model", C.c_void_p), ("cam_params", C.c_void_p),
+                ("cam_const_mask", C.c_void_p), ("qvec", C.c_void_p), ("tvec", C.c_void_p), ("obs_begin", C.c_void_p),
+                ("xyz", C.c_void_p), ("obs_patch", C.c_void_p), ("refs", C.c_void_p), ("patch_blocks", C.c_void_p),
+                ("patch_counts", C.c_void_p), ("corner", C.c_void_p), ("scale", C.c_void_p),
+                ("upsampling_factor", C.c_double), ("ph", C.c_int32), ("pw", C.c_int32), ("channels", C.c_int32),
+                ("patch_dtype", C.c_int32), ("max_wave_bytes", C.c_double)]
+
+
+class QBAResult(C.Structure):          # pxr_qba_result
+    _fields_ = [("status", C.c_int32), ("num_residual_blocks", C.c_int32), ("initial_cost", C.c_double),
+                ("final_cost", C.c_double), ("num_iterations", C.c_int32), ("num_successful_steps", C.c_int32),
+                ("num_unsuccessful_steps", C.c_int32), ("termination_type", C.c_int32),
+                ("block_evaluations", C.c_int64)]
+
+
+class QBABatch:
+    """numpy arrays of a batch of query bundle adjustments + the ctypes view (pxr_qba_desc).  Per query: camera model,
+    params [12] (in/out), constancy mask, qvec / tvec (in/out), a patch block [n_q, H, W, C] (host numpy array or
+    anything with `.ptr` / __cuda_array_interface__ in device memory) with its corners and scales; per residual block:
+    xyz, patch index within its query's block and one fp64 reference descriptor."""
+
+    def __init__(self, cam_model, cam_params, cam_const_mask, qvec, tvec, obs_begin, xyz, obs_patch, refs,
+                 patch_blocks, corner, scale, upsampling_factor=1.0, max_wave_bytes=0.0):
+        self.cam_model = _as(cam_model, np.int32)
+        nq = len(self.cam_model)
+        cp = np.zeros((nq, PXR_MAX_CAM_PARAMS), np.float64)
+        for i in range(nq):
+            p = np.asarray(cam_params[i], np.float64).reshape(-1)
+            cp[i, :len(p)] = p
+        self.cam_params = cp
+        self.cam_const_mask = _as(cam_const_mask, np.uint32)
+        self.qvec = _as(qvec, np.float64, (-1, 4)).copy()
+        self.tvec = _as(tvec, np.float64, (-1, 3)).copy()
+        self.obs_begin = _as(obs_begin, np.int64)
+        m = int(self.obs_begin[-1]) if len(self.obs_begin) else 0
+        self.xyz = _as(xyz, np.float64, (-1, 3)) if m else np.zeros((0, 3))
+        self.obs_patch = _as(obs_patch, np.int64) if m else np.zeros(0, np.int64)
+        self.refs = np.ascontiguousarray(refs, np.float64) if m else None
+        if len(patch_blocks) != nq:
+            raise ValueError("one patch block per query")
+        self.patch_blocks = list(patch_blocks)
+        ptrs, counts, shape, dtype = [], [], None, None
+        for b in self.patch_blocks:
+            cai = getattr(b, "__cuda_array_interface__", None)
+            if getattr(b, "ptr", None) is not None:
+                p, shp, dt = int(b.ptr), tuple(b.shape), np.dtype(b.dtype)
+            elif cai is not None:
+                p, shp, dt = int(cai["data"][0]), tuple(cai["shape"]), np.dtype(cai["typestr"])
+            else:
+                if b.dtype not in DTYPE_IDS or not b.flags["C_CONTIGUOUS"] or b.ndim != 4:
+                    raise ValueError("patch blocks must be C-contiguous [N,H,W,C] f16/f32/f64 arrays")
+                p, shp, dt = b.ctypes.data, tuple(b.shape), np.dtype(b.dtype)
+            if shape is not None and (shp[1:] != shape or dt != dtype):
+                raise ValueError("patch blocks must share one dtype and patch shape")
+            shape, dtype = shp[1:], dt
+            ptrs.append(p); counts.append(shp[0])
+        self._ptrs = (C.c_void_p * max(nq, 1))(*ptrs)
+        self.patch_counts = np.array(counts, np.int64)
+        self.ph, self.pw, self.channels = shape if shape is not None else (1, 1, 8)
+        self.patch_dtype = DTYPE_IDS[dtype] if dtype is not None else 0
+        self.corner = _as(corner, np.int32, (-1, 2))
+        self.scale = _as(scale, np.float64, (-1, 2))
+        self.upsampling_factor = float(upsampling_factor)
+        self.max_wave_bytes = float(max_wave_bytes)
+
+    @property
+    def n_queries(self):
+        return len(self.cam_model)
+
+    def desc(self):
+        d = QBADesc()
+        d.n_queries = self.n_queries
+        d.cam_model = _ptr(self.cam_model); d.cam_params = _ptr(self.cam_params)
+        d.cam_const_mask = _ptr(self.cam_const_mask); d.qvec = _ptr(self.qvec); d.tvec = _ptr(self.tvec)
+        d.obs_begin = _ptr(self.obs_begin); d.xyz = _ptr(self.xyz); d.obs_patch = _ptr(self.obs_patch)
+        d.refs = _ptr(self.refs)
+        d.patch_blocks = C.cast(self._ptrs, C.c_void_p); d.patch_counts = _ptr(self.patch_counts)
+        d.corner = _ptr(self.corner); d.scale = _ptr(self.scale)
+        d.upsampling_factor = self.upsampling_factor
+        d.ph, d.pw, d.channels, d.patch_dtype = self.ph, self.pw, self.channels, self.patch_dtype
+        d.max_wave_bytes = self.max_wave_bytes
+        return d
+
+
 def make_summary(capacity=256):
     s = Summary()
     buf = (IterationSummary * max(capacity, 1))()

@@ -193,6 +193,60 @@ def ba_run(problem, interp=None, options=None, ctx=None, capacity=512):
     return _capi.summary_to_dict(s)
 
 
+def qba_run(batch, interp=None, options=None, ctx=None, capacity=0):
+    """pxr_qba_run: solves every query of a _capi.QBABatch and writes the refined qvec / tvec / cam_params back into
+    it (in place).  -> (list of per-query dicts with the pxr_qba_result fields and, with capacity > 0, `iterations`,
+    dict(n_waves, h2d_bytes, solve_time_s, total_time_s, kernel_launches, message))"""
+    ctx = ctx or _capi.default_context()
+    interp = interp or _capi.default_interp()
+    options = options or _capi.default_ba_options(use_inner_iterations=0)
+    d = batch.desc()
+    nq = batch.n_queries
+    res = (_capi.QBAResult * max(nq, 1))()
+    its = (_capi.IterationSummary * max(nq * capacity, 1))()
+    nw = C.c_int32()
+    tot = _capi.make_summary(0)
+    _capi.check(ctx.lib.pxr_qba_run(ctx.handle, C.byref(d), C.byref(interp), C.byref(options), res,
+                                    its if capacity else None, int(capacity), C.byref(nw), C.byref(tot)))
+    out = []
+    for q in range(nq):
+        r = {f[0]: getattr(res[q], f[0]) for f in _capi.QBAResult._fields_}
+        if capacity:
+            k = min(r["num_iterations"], capacity)
+            r["iterations"] = [{f[0]: getattr(its[q * capacity + i], f[0]) for f in _capi.IterationSummary._fields_}
+                               for i in range(k)]
+        out.append(r)
+    t = _capi.summary_to_dict(tot)
+    return out, dict(n_waves=nw.value, h2d_bytes=t["h2d_bytes"], solve_time_s=t["solve_time_s"],
+                     total_time_s=t["total_time_s"], kernel_launches=t["kernel_launches"], message=t["message"])
+
+
+def qba_plan_waves(batch):
+    """pxr_qba_plan_waves: (first query of every wave + the end, uploaded bytes per wave) — host computation"""
+    lib = _capi.load_lib()
+    d = batch.desc()
+    nq = batch.n_queries
+    begin = np.zeros(nq + 1, np.int32); nbytes = np.zeros(max(nq, 1)); nw = C.c_int32()
+    _capi.check(lib.pxr_qba_plan_waves(C.byref(d), _p(begin), C.byref(nw), _p(nbytes)))
+    return begin[:nw.value + 1].copy(), nbytes[:nw.value].copy()
+
+
+def qba_debug_linearize(batch, interp=None, options=None, ctx=None):
+    """pxr_qba_debug_linearize: every query's cost, J^T J (lower, [nq, 18, 18]) and J^T r ([nq, 18]) at the batch's
+    parameters, and every block's projection xy [n_obs, 2] and K1 record [n_obs, 8]"""
+    ctx = ctx or _capi.default_context()
+    interp = interp or _capi.default_interp()
+    options = options or _capi.default_ba_options(use_inner_iterations=0)
+    d = batch.desc()
+    nq, m = batch.n_queries, int(batch.obs_begin[-1])
+    out = dict(cost=np.zeros(nq), H=np.zeros((nq, 18, 18)), g=np.zeros((nq, 18)), xy=np.zeros((m, 2)),
+               rec=np.zeros((m, 8)))
+    _capi.check(ctx.lib.pxr_qba_debug_linearize(ctx.handle, C.byref(d), C.byref(interp), C.byref(options),
+                                                _p(out["cost"]), _p(out["H"]), _p(out["g"]), _p(out["xy"]),
+                                                _p(out["rec"])))
+    return out
+
+
 class PinnedArray:
     """A numpy array in pinned (page-locked, device-mapped) host memory from pxr_host_alloc_pinned: the patch source
     pxr_ba_run reads tap windows from directly (window residency, csrc/pxr_resident.cuh) and full-rate DMA otherwise.

@@ -216,3 +216,94 @@ class QueryBundleOptimizer:
 
     def summary(self):
         return self._summary
+
+    # ---- batched: many queries in one pxr_qba_run
+    def pack_batch(self, queries, max_wave_bytes=0.0):
+        """the per-query arrays build_problem makes, concatenated into one _capi.QBABatch.  `queries` is a list of the
+        argument tuples run takes, (qvec, tvec, camera, points3D, fmap, references[, inliers[, patch_idxs]]); feature
+        maps may hold host (numpy) or device patches (DevicePatches, read in place)."""
+        self.interp.validate_for_device()
+        model, params, masks, qv, tv, begin, xyz, refs, obs_patch, blocks, corners, scales = ([] for _ in range(12))
+        begin.append(0)
+        channels = None
+        o = self.options
+        for args in queries:
+            qvec, tvec, camera, points3D, fmap, references = args[:6]
+            inliers = args[6] if len(args) > 6 else None
+            patch_idxs = args[7] if len(args) > 7 else None
+            n = len(points3D)
+            if len(references) != n:
+                raise ValueError("references.size() != points3D.size()")
+            if patch_idxs is not None and len(patch_idxs) != n:
+                raise ValueError("patch_idxs.size() != points3D.size()")
+            if len(self.interp.nodes) != 1 or fmap.channels not in (8, 16, 32, 64, 128, 256):
+                raise ValueError("Unsupported dimensions (CHANNELS,N_NODES).")
+            if channels is not None and fmap.channels != channels:
+                raise ValueError("every query of a batch must have the same channel count")
+            channels = fmap.channels
+            for i in range(n):
+                if inliers is not None and not inliers[i]:
+                    continue
+                pi = fmap.local_index(i if patch_idxs is None else patch_idxs[i])
+                for dsc in _descriptors_of(references[i], fmap.channels):   # one residual block per reference descriptor
+                    xyz.append(np.asarray(points3D[i], np.float64).reshape(3)); refs.append(dsc); obs_patch.append(pi)
+            begin.append(len(xyz))
+            m = int(camera.model_id)
+            focal, pp, extra = _capi.CAMERA_PARAM_GROUPS[m]
+            if not (o.refine_focal_length or o.refine_principal_point or o.refine_extra_params):
+                masks.append(0xFFFFFFFF)
+            else:
+                masks.append((0 if o.refine_focal_length else focal) | (0 if o.refine_principal_point else pp) |
+                             (0 if o.refine_extra_params else extra))
+            model.append(m); params.append(np.asarray(camera.params, np.float64))
+            qv.append(np.asarray(qvec, np.float64).reshape(4)); tv.append(np.asarray(tvec, np.float64).reshape(3))
+            blocks.append(fmap.patches)
+            corners.append(np.asarray(fmap.corners, np.int32).reshape(-1, 2))
+            scales.append(np.tile(fmap.scale, (fmap.size(), 1)))
+        return _capi.QBABatch(model, params, masks, np.array(qv).reshape(-1, 4), np.array(tv).reshape(-1, 3), begin,
+                              np.array(xyz).reshape(-1, 3), obs_patch, np.array(refs) if refs else None, blocks,
+                              np.concatenate(corners) if corners else np.zeros((0, 2), np.int32),
+                              np.concatenate(scales) if scales else np.zeros((0, 2)), max_wave_bytes=max_wave_bytes)
+
+    def run_batch(self, queries, max_wave_bytes=0.0):
+        """run() for every query of `queries` (argument tuples as pack_batch takes them) in one pxr_qba_run: each
+        query's qvec / tvec / camera.params are refined IN PLACE.  -> one bool per query (False: no residual block).
+        summaries() gives each query's summary; its total_time_s and solve_time_s are those of the whole batch (the
+        queries are solved together), which is also what the one "QBA Time" log line per batch reports.  A query whose
+        initial cost is not finite raises the error run() would raise, naming the query, after every other query has
+        been written back."""
+        queries = list(queries)
+        batch = self.pack_batch(queries, max_wave_bytes)
+        so = self.solver_options()
+        ic = _capi.default_interp(self.interp.l2_normalize, self.interp.use_float_simd)
+        res, tot = _engine.qba_run(batch, ic, so, capacity=max(1, int(so.max_num_iterations) + 1))
+        self._summaries, ok, failed = [], [], []
+        for k, (args, r) in enumerate(zip(queries, res)):
+            if r["num_residual_blocks"] == 0 or r["status"] != _capi.PXR_OK:
+                self._summaries.append(None); ok.append(False)
+                if r["num_residual_blocks"]:
+                    failed.append(k)
+                continue
+            qvec, tvec, camera = args[:3]
+            np.asarray(qvec).reshape(-1)[:] = batch.qvec[k]
+            np.asarray(tvec).reshape(-1)[:] = batch.tvec[k]
+            camera.params[:] = batch.cam_params[k, :len(camera.params)]
+            nres = max(1, r["num_residual_blocks"] * batch.channels)
+            s = dict(initial_cost=r["initial_cost"], final_cost=r["final_cost"],
+                     num_residual_blocks=r["num_residual_blocks"], num_residuals=r["num_residual_blocks"] * batch.channels,
+                     num_successful_steps=r["num_successful_steps"], num_unsuccessful_steps=r["num_unsuccessful_steps"],
+                     num_inner_iteration_steps=0, termination_type=r["termination_type"],
+                     total_time_s=tot["total_time_s"], solve_time_s=tot["solve_time_s"], num_iterations=r["num_iterations"],
+                     block_evaluations=r["block_evaluations"], iterations=r.get("iterations", []))
+            self._summaries.append(_Summary(s, num_residuals_reduced=nres))
+            logger.info("QBA query %d: cost change: %.6g --> %.6g", k, np.sqrt(r["initial_cost"] / nres),
+                        np.sqrt(r["final_cost"] / nres))
+            ok.append(True)
+        logger.info("QBA Time: %.4gs for %d queries in %d waves", tot["total_time_s"], len(queries), tot["n_waves"])
+        if failed:
+            raise _capi.PxrError("pxr status %d: query %d: initial cost is not finite" % (_capi.PXR_ERR_NUMERIC, failed[0]))
+        return ok
+
+    def summaries(self):
+        """per-query summaries of the last run_batch (None for a query that was not solved)"""
+        return getattr(self, "_summaries", [])

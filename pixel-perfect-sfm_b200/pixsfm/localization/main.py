@@ -117,6 +117,27 @@ class QueryBundleAdjuster:
             self.refine(qvec, tvec, camera, points3D, fmaps[level], references[level], inliers=inliers,
                         point2D_idxs=point2D_idxs)
 
+    def refine_batch(self, queries, max_wave_bytes=0.0):
+        """refine() for every query of `queries`, tuples (qvec, tvec, camera, points3D, fmap, references[, inliers[,
+        point2D_idxs]]), in one batched solve (QueryBundleOptimizer.run_batch) -> one bool per query"""
+        return self.solver.run_batch(queries, max_wave_bytes)
+
+    def refine_multilevel_batch(self, queries, max_wave_bytes=0.0):
+        """refine_multilevel() for every query of `queries`, tuples (qvec, tvec, camera, points3D, fmaps, references[,
+        inliers[, point2D_idxs]]) with one fmap and one reference list per level: each level is one batched solve that
+        starts from the previous level's result"""
+        queries = list(queries)
+        if not queries:
+            return
+        n_levels = len(queries[0][4])
+        for q in queries:
+            if len(q[4]) != len(q[5]):
+                raise ValueError("one reference list per feature level is required")
+            if len(q[4]) != n_levels:
+                raise ValueError("every query of a batch must have the same number of feature levels")
+        for level in level_order(self.conf.level_indices, n_levels):
+            self.refine_batch([tuple(q[:4]) + (q[4][level], q[5][level]) + tuple(q[6:]) for q in queries], max_wave_bytes)
+
 
 def compute_reprojection_errors(pnp_points2D, pnp_points3D, qvec, tvec, camera):
     """pixel distance between every 2D point and the projection of its 3D point (reference main.py:96-102)"""
@@ -242,12 +263,39 @@ class QueryLocalizer:
         `pnp_point2D_idxs[k]` with 3D point `pnp_points3D_id[k]`.  Returns the pose dict of the PnP step with the refined
         pose, `inliers` / `num_inliers` recomputed from it, and (an addition) `keypoints`: the refined 2D points of the
         correspondences."""
+        st = self._localize_begin(keypoints, pnp_point2D_idxs, pnp_points3D_id, query_camera, image_path, query_fmaps,
+                                  pose_estimator)
+        if "result" in st:
+            return st["result"]
+        if self.conf.QBA.apply:
+            self.query_bundle_adjuster.refine_multilevel(*self._qba_args(st))
+        return self._localize_end(st)
+
+    def localize_batch(self, queries, max_wave_bytes=0.0):
+        """localize() for every entry of `queries` (dicts of localize's keyword arguments): QKA and PnP per query as
+        localize runs them, then one batched QBA solve per feature level over every query that has a pose, then the
+        per-query inlier recomputation.  Returns the list of pose dicts localize would return."""
+        states = [self._localize_begin(**q) for q in queries]
+        live = [st for st in states if "result" not in st]
+        if self.conf.QBA.apply and live:
+            self.query_bundle_adjuster.refine_multilevel_batch([self._qba_args(st) for st in live], max_wave_bytes)
+        return [st["result"] if "result" in st else self._localize_end(st) for st in states]
+
+    @staticmethod
+    def _qba_args(st):
+        pose = st["pose"]
+        return (pose["qvec"], pose["tvec"], st["camera"], st["points3D"], st["fmaps"], st["references"], list(st["inliers"]),
+                st["point2D_idxs"])
+
+    def _localize_begin(self, keypoints, pnp_point2D_idxs, pnp_points3D_id, query_camera, image_path=None, query_fmaps=None,
+                        pose_estimator=None):
+        """localize up to the QBA step: {"result": pose dict} when it ends early, else the state _localize_end takes"""
         if len(pnp_point2D_idxs) != len(pnp_points3D_id):
             raise ValueError("one 3D point id per 2D index is required")
         if image_path is None and query_fmaps is None:
             raise ValueError("image_path or query_fmaps are required")
         if len(pnp_point2D_idxs) == 0:
-            return {"success": False}
+            return {"result": {"success": False}}
         pnp_point2D_idxs = [int(i) for i in pnp_point2D_idxs]
         pnp_points3D = [np.asarray(self.reconstruction.points3D[p3D_id].xyz, np.float64) for p3D_id in pnp_points3D_id]
         keypoints = np.array(keypoints, dtype=np.float64)
@@ -265,7 +313,7 @@ class QueryLocalizer:
                                                            point2D_idxs=pnp_point2D_idxs)
         pose_dict = self._absolute_pose(pnp_points2D, pnp_points3D, query_camera, pose_estimator)
         if not pose_dict.get("success", False):
-            return pose_dict
+            return {"result": pose_dict}
         inliers = pose_dict.get("inliers", [True] * len(pnp_points3D))
         if self.conf.unique_inliers:                          # None / False: keep what PnP says
             if self.conf.unique_inliers == "random":
@@ -277,13 +325,14 @@ class QueryLocalizer:
             else:
                 from .. import logger
                 logger.warning("Unknown unique_inlier method %s.", self.conf.unique_inliers)
-        if self.conf.QBA.apply:
-            self.query_bundle_adjuster.refine_multilevel(pose_dict["qvec"], pose_dict["tvec"], query_camera, pnp_points3D,
-                                                         query_fmaps, query_references, inliers=list(inliers),
-                                                         point2D_idxs=pnp_point2D_idxs)
-        errors = compute_reprojection_errors(pnp_points2D, pnp_points3D, pose_dict["qvec"], pose_dict["tvec"], query_camera)
+        return {"pose": pose_dict, "camera": query_camera, "points2D": pnp_points2D, "points3D": pnp_points3D,
+                "fmaps": query_fmaps, "references": query_references, "inliers": inliers, "point2D_idxs": pnp_point2D_idxs}
+
+    def _localize_end(self, st):
+        pose_dict = st["pose"]
+        errors = compute_reprojection_errors(st["points2D"], st["points3D"], pose_dict["qvec"], pose_dict["tvec"], st["camera"])
         max_error = self.conf.PnP.estimation.ransac.max_error
         pose_dict["inliers"] = [err < max_error for err in errors]
         pose_dict["num_inliers"] = sum(pose_dict["inliers"])
-        pose_dict["keypoints"] = pnp_points2D
+        pose_dict["keypoints"] = st["points2D"]
         return pose_dict
