@@ -340,6 +340,9 @@ int pxr_ba_debug_eval_list(pxr_ba* ba, const int64_t* list, int64_t n, int count
  * count_on_device as in pxr_ba_debug_eval_list. */
 int pxr_ba_debug_project_point(pxr_ba* ba, const int64_t* list, int64_t n, int count_on_device, double* uv, double* jpt,
                                double* uv_full);
+/* K0 over all observations at the current parameters (tests): jac = 0 the cost-only projection, 1 the one with
+ * Jacobians.  uv [n_obs][2] (patch pixels), xy [n_obs][2] (image pixels).  Any output may be NULL. */
+int pxr_ba_debug_project(pxr_ba* ba, int jac, double* uv, double* xy);
 /* Batched inner iterations run with capture on (enable = 1) keep each round's lists (tests; the host waits for every
  * round).  pxr_ba_debug_inner_round_lists then reads round `round` of the most recent call: *n_points / *n_obs its list
  * lengths, plist [*n_points] its points, list [*n_obs] its observations, active [*n_points] 1 where the round's step

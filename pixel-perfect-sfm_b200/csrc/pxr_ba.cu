@@ -998,8 +998,8 @@ int BA::compute_step(double radius, bool* valid, double* model_cost_change) {
   return PXR_OK;
 }
 
-// candidate (other set) = Plus(current, delta); returns ||step|| and ||x|| (ambient)
-int BA::apply_step(double* step_norm, double* x_norm) {
+// candidate (other set) = Plus(current, delta); ||step||^2 and ||x||^2 (ambient; point parts, camera parts) to scalars[5..8]
+int BA::apply_step() {
   PlusArgs a;
   a.n_cameras = n_cameras; a.n_images = n_images; a.n_points = n_points;
   a.cam_model = cam_model.p; a.cam_mask = cam_mask.p; a.tmask = tmask.p;
@@ -1016,13 +1016,6 @@ int BA::apply_step(double* step_norm, double* x_norm) {
     for (int k = 0; k < 4; ++k) PXR_LAUNCH(ctx, det_reduce_add_kernel, 1, 1024, 0, det_scal_part.p, cdiv(n, 128), 4, k, a.acc + 1 + k);
   PXR_CUDA(cudaGetLastError());
   if (!block_mode) PXR_TRY(allreduce_f64(ctx, scalars.p + 5, 2));  // point parts are sharded, camera parts replicated (block mode: scalar exchange)
-  if (step_norm || x_norm) {
-    double v[4];
-    PXR_CUDA(cudaMemcpyAsync(v, scalars.p + 5, 32, cudaMemcpyDeviceToHost, ctx->stream));
-    PXR_CUDA(cudaStreamSynchronize(ctx->stream));
-    if (step_norm) *step_norm = std::sqrt(v[0] + v[2]);
-    if (x_norm) *x_norm = std::sqrt(v[1] + v[3]);
-  }
   return PXR_OK;
 }
 
@@ -1089,14 +1082,14 @@ int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long l
 }
 
 // Inner iterations, batched: see pxr_inner.cuh.  Same state machine as ba_inner_kernel.
-// Round 0's lists come from every variable point; from then on a round is three launches (K0, K1, inner_step_kernel) and
-// the step kernel builds the next round's lists.  Lists alternate between two buffers, counters rotate through three sets
+// Round 0's lists come from every variable point (round 0 itself evaluates every observation); from then on a round is
+// three launches (K0, K1, inner_step_kernel) and the step kernel builds the next round's lists.  Lists alternate between two buffers, counters rotate through three sets
 // (the step kernel of round r appends to set r+1 and zeroes set r+2, which no launch of round r touches).  The rounds are
 // enqueued WITHOUT waiting for the host: each step kernel copies its round's list lengths to a host-mapped slot, tagged
 // with the call's epoch, and the host stops enqueuing once a round two behind has reported an empty list (the two extra
 // rounds find nothing to do).
 constexpr int kInnerRounds = 53;
-int BA::inner_rounds(int set) {
+int BA::inner_rounds(int set, double* trial_cost) {
   cudaStream_t s = ctx->stream;
   volatile unsigned long long* slots = inner_cnt_host;
   const unsigned long long epoch = ++inner_epoch;
@@ -1152,7 +1145,15 @@ int BA::inner_rounds(int set) {
     a.publish = inner_cnt_dev + 3 * round;
     cudaEvent_t* ev = inner_rounds_timed ? inner_round_timed[round].data() : nullptr;
     if (ev) PXR_CUDA(cudaEventRecord(ev[0], s));
-    PXR_TRY(eval_list(set, inner_list[cur].p, n_obs, cnt, false, ev ? ev[1] : nullptr, ev ? ev[2] : nullptr, bound_obs));
+    if (round == 0) {
+      // every observation, those of constant points included, so that the records also give the cost at the starting
+      // point: reduced here, before the step kernel, with the kernels and partial order of fm_cost's full pass.  Under
+      // window residency a batch with violations is run again from round 0, which overwrites the cost.
+      PXR_TRY(eval_list(set, nullptr, n_obs, nullptr, false, ev ? ev[1] : nullptr, ev ? ev[2] : nullptr));
+      if (trial_cost) PXR_TRY(fm_cost(trial_cost));
+    } else {
+      PXR_TRY(eval_list(set, inner_list[cur].p, n_obs, cnt, false, ev ? ev[1] : nullptr, ev ? ev[2] : nullptr, bound_obs));
+    }
     const unsigned sgrid = (unsigned)std::min<int64_t>(cdiv(bound_pts, 128), (int64_t)ctx->sm_count * 8);
     PXR_LAUNCH(ctx, inner_step_kernel, sgrid, 128, 0, a, round == 0 ? 0 : 1);
     if (ev) PXR_CUDA(cudaEventRecord(ev[3], s));
@@ -1189,8 +1190,8 @@ int BA::capture_round_active() {
   return PXR_OK;
 }
 
-int BA::inner_iterations_batched(int set) {
-  if (n_points == 0 || n_obs == 0) return PXR_OK;
+int BA::inner_iterations_batched(int set, double* trial_cost) {
+  if (n_points == 0 || n_obs == 0) return trial_cost ? fm_cost(trial_cost) : PXR_OK;
   StageScope stg(this, 9);
   cudaStream_t s = ctx->stream;
   if (!inner_state.p) {
@@ -1202,13 +1203,13 @@ int BA::inner_iterations_batched(int set) {
     std::memset(inner_cnt_host, 0, (size_t)kInnerRounds * 3 * sizeof(unsigned long long));
     PXR_CUDA(cudaHostGetDevicePointer((void**)&inner_cnt_dev, inner_cnt_host, 0));
   }
-  if (!resident) return inner_rounds(set);
+  if (!resident) return inner_rounds(set, trial_cost);
   // window residency: an observation may leave its window in any round and nobody looks before the rounds are over — keep
   // the starting points, and if something was reported fetch those patches and run the rounds again from the start
   if (!inner_snapshot.p) PXR_TRY(inner_snapshot.alloc((size_t)n_points * 3));
   PXR_CUDA(cudaMemcpyAsync(inner_snapshot.p, X[set].p, (size_t)n_points * 24, cudaMemcpyDeviceToDevice, s));
   for (;;) {
-    PXR_TRY(inner_rounds(set));
+    PXR_TRY(inner_rounds(set, trial_cost));
     int64_t n_fixed = 0;
     PXR_TRY(resident_fix(&n_fixed));
     if (n_fixed == 0) break;
@@ -1217,8 +1218,12 @@ int BA::inner_iterations_batched(int set) {
   return PXR_OK;
 }
 
-int BA::inner_iterations(int set) {
-  if (!use_monolithic_inner) return inner_iterations_batched(set);
+int BA::inner_iterations(int set, double* trial_cost) {
+  if (!use_monolithic_inner) return inner_iterations_batched(set, trial_cost);
+  if (trial_cost) {     // the monolithic kernel leaves no records behind: the cost takes a pass of its own
+    PXR_TRY(project(set, false, nullptr));
+    PXR_TRY(fm(0, nullptr, trial_cost));
+  }
   InnerArgs a;
   a.n_points = n_points; a.point_off = point_off.p; a.pt_begin = pt_begin.p;
   a.obs_img = obs_img.p; a.obs_patch = obs_patch.p; a.img_cam = img_cam.p; a.cam_model = cam_model.p;
@@ -1233,21 +1238,21 @@ int BA::inner_iterations(int set) {
   return launch_inner(ctx, dtype, C, interp.use_float_simd != 0, a);
 }
 
-int BA::step_norm_between_sets(double* out) {
+// ||set 0 - set 1||^2 (ambient), the step after inner iterations: points to scalars[11], cameras to scalars[12].  Only
+// enqueued; the drivers read it with the iteration's other scalars.
+int BA::step_norm_between_sets() {
   cudaStream_t s = ctx->stream;
   PXR_CUDA(cudaMemsetAsync(scalars.p + 11, 0, 16, s));
-  auto run = [&](const double* a, const double* b, int64_t n, double* acc) {
-    if (n > 0) PXR_LAUNCH(ctx, diff_norm_kernel, (unsigned)cdiv(n, 256), 256, 0, a, b, n, acc);
+  auto run = [&](const double* a, const double* b, int64_t n, double* acc) -> int {
+    if (n <= 0) return PXR_OK;
+    PXR_LAUNCH(ctx, diff_norm_kernel, (unsigned)cdiv(n, 256), 256, 0, a, b, n, acc, deterministic ? det_scal_part.p : nullptr);
+    if (deterministic) PXR_LAUNCH(ctx, det_reduce_add_kernel, 1, 1024, 0, det_scal_part.p, cdiv(n, 256), 1, 0, acc);
+    return PXR_OK;
   };
-  run(cam[0].p, cam[1].p, (int64_t)n_cameras * kMaxK, scalars.p + 12);
-  run(q[0].p, q[1].p, (int64_t)n_images * 4, scalars.p + 12);
-  run(t[0].p, t[1].p, (int64_t)n_images * 3, scalars.p + 12);
-  run(X[0].p, X[1].p, n_points * 3, scalars.p + 11);
-  PXR_TRY(allreduce_f64(ctx, scalars.p + 11, 1));
-  double v[2] = {0, 0};
-  PXR_CUDA(cudaMemcpyAsync(v, scalars.p + 11, 16, cudaMemcpyDeviceToHost, s));
-  PXR_CUDA(cudaStreamSynchronize(s));
-  *out = std::sqrt(v[0] + v[1]);
+  PXR_TRY(run(cam[0].p, cam[1].p, (int64_t)n_cameras * kMaxK, scalars.p + 12));
+  PXR_TRY(run(q[0].p, q[1].p, (int64_t)n_images * 4, scalars.p + 12));
+  PXR_TRY(run(t[0].p, t[1].p, (int64_t)n_images * 3, scalars.p + 12));
+  PXR_TRY(run(X[0].p, X[1].p, n_points * 3, scalars.p + 11));
   return PXR_OK;
 }
 
@@ -1476,49 +1481,52 @@ int BA::lm_iterate(int max_iteration) {
     }
     lm.num_invalid = 0;
 
-    double step_norm = 0, x_norm = 0, candidate_cost = 0;
-    const bool speculate = !lm.inner_enabled && !env.no_speculation;
-    // the norms of the step are read back together with the trial cost (one host round trip instead of two)
-    if (speculate) PXR_TRY(apply_step(nullptr, nullptr)); else PXR_TRY(apply_step(&step_norm, &x_norm));
-    // Trial point.  Ceres evaluates the cost here and, if the step is accepted, evaluates residuals AND Jacobians
-    // again at the same point.  Both passes stream the same patch windows, so when no inner iterations will move
-    // the point afterwards the Jacobian-mode pass is run right away into the alternate buffer set, which saves one
-    // cost-only pass per accepted step; a rejected step merely discards it.
+    // Trial point.  Ceres evaluates the cost here and, if the step is accepted, residuals AND Jacobians again at the
+    // point it moves to.  Both passes stream the same patch windows, so with speculation (DESIGN §4) the pass at that
+    // point runs in Jacobian mode right away, into the alternate buffer set; a rejected step merely discards it.
+    // Without inner iterations that pass is the trial pass.  With them the trial cost comes from inner-iteration round 0,
+    // which evaluates every observation at the trial point, and the pass after the rounds is the one at the final point.
+    // Ceres skips inner iterations when the trial cost is not finite; here they run regardless and their result is
+    // ignored (such a step is rejected, and its parameter set with it).  The costs and the norms of the step come back
+    // in one host round trip.  PXR_NO_SPECULATION: cost-only passes, and the accepted point is evaluated again.
+    const bool speculate = !env.no_speculation;
+    const bool ran_inner = lm.inner_enabled;
+    const bool round0_cost = ran_inner && speculate;
+    PXR_TRY(apply_step());
     swap_sets();
-    int rc = PXR_OK;
-    if (speculate) {
-      rc = project(1 - cur, true, nullptr);
-      if (rc == PXR_OK) rc = fm(1, nullptr, scalars.p + 0);
-      if (rc == PXR_OK) rc = allreduce_f64(ctx, scalars.p + 0, 1);
-      if (rc == PXR_OK) {
-        double nv[4] = {0, 0, 0, 0};
-        cudaError_t e = cudaMemcpyAsync(&candidate_cost, scalars.p + 0, 8, cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(nv, scalars.p + 5, 32, cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess) rc = fail(PXR_ERR_CUDA, "trial evaluation failed: %s", cudaGetErrorString(e));
-        step_norm = std::sqrt(nv[0] + nv[2]); x_norm = std::sqrt(nv[1] + nv[3]);
-      }
-    } else {
-      rc = evaluate(1 - cur, false, &candidate_cost);
+    int rc = round0_cost ? inner_iterations(1 - cur, scalars.p + 0) : project(1 - cur, speculate, nullptr);
+    if (rc == PXR_OK && !round0_cost) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
+    if (ran_inner) {
+      if (rc == PXR_OK && !round0_cost) rc = inner_iterations(1 - cur);
+      if (rc == PXR_OK) rc = project(1 - cur, speculate, nullptr);
+      if (rc == PXR_OK) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 1);
+      if (rc == PXR_OK) rc = step_norm_between_sets();
+      if (rc == PXR_OK) rc = allreduce_f64(ctx, scalars.p + 11, 1);
+    }
+    if (rc == PXR_OK) rc = allreduce_f64(ctx, scalars.p + 0, ran_inner ? 2 : 1);
+    double v[13] = {};     // [0] trial cost, [1] cost after the inner iterations, [5..8] apply_step's norms, [11..12] the step after them
+    if (rc == PXR_OK) {
+      cudaError_t e = cudaMemcpyAsync(v, scalars.p, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+      if (e != cudaSuccess) rc = fail(PXR_ERR_CUDA, "trial evaluation failed: %s", cudaGetErrorString(e));
     }
     if (rc != PXR_OK) { swap_sets(); return rc; }
-    if (!std::isfinite(candidate_cost)) candidate_cost = std::numeric_limits<double>::max();
+    double candidate_cost = std::isfinite(v[0]) ? v[0] : std::numeric_limits<double>::max();
+    double step_norm = std::sqrt(v[5] + v[7]);
+    const double x_norm = std::sqrt(v[6] + v[8]);
+    const double next_cost = ran_inner ? v[1] : candidate_cost;     // the cost of the pass left in the alternate set
 
     bool inner_useful = false;
-    if (lm.inner_enabled && candidate_cost < std::numeric_limits<double>::max()) {
+    if (ran_inner && candidate_cost < std::numeric_limits<double>::max()) {
       ++lm.n_inner;
-      rc = inner_iterations(1 - cur);
-      double inner_cost = 0;
-      if (rc == PXR_OK) rc = evaluate(1 - cur, false, &inner_cost);
-      if (rc != PXR_OK) { swap_sets(); return rc; }
+      const double inner_cost = v[1];
       if (std::isfinite(inner_cost)) {
         model_cost_change += candidate_cost - inner_cost;
         inner_useful = inner_cost < lm.x_cost;
         const double rel = 1.0 - inner_cost / candidate_cost;
         lm.inner_enabled = rel > opt.inner_iteration_tolerance;
         candidate_cost = inner_cost;
-        rc = step_norm_between_sets(&step_norm);
-        if (rc != PXR_OK) { swap_sets(); return rc; }
+        step_norm = std::sqrt(v[11] + v[12]);
       }
     }
     swap_sets();   // back: uv/obs_out/juv = linearisation at the current point again
@@ -1537,7 +1545,7 @@ int BA::lm_iterate(int max_iteration) {
       if (speculate && candidate_cost < std::numeric_limits<double>::max()) {
         swap_sets();                 // the speculative pass IS the linearisation at the new point
         PXR_TRY(build());
-        lm.x_cost = candidate_cost;
+        lm.x_cost = next_cost;
       } else {
         PXR_TRY(evaluate(cur, true, &lm.x_cost));
       }
@@ -1934,6 +1942,22 @@ int pxr_ba_debug_project_point(pxr_ba* ba, const int64_t* list, int64_t n, int c
   }
   PXR_CUDA(cudaMemcpyAsync(uv, b->uv.p, (size_t)b->n_obs * 16, cudaMemcpyDeviceToHost, s));
   PXR_CUDA(cudaMemcpyAsync(jpt, b->inner_jpt.p, (size_t)b->n_obs * 48, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  return PXR_OK;
+}
+
+// K0 over all observations at the current parameters, cost-only (jac = 0) or with Jacobians (tests): uv and xy
+int pxr_ba_debug_project(pxr_ba* ba, int jac, double* uv, double* xy) {
+  if (!ba || (jac != 0 && jac != 1)) return fail(PXR_ERR_INVALID_ARGUMENT, "bad arguments");
+  BA* b = reinterpret_cast<BA*>(ba);
+  pxr_ctx* ctx = b->ctx;
+  cudaStream_t s = ctx->stream;
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  DevBuf<double> dxy;
+  if (xy) PXR_TRY(dxy.alloc((size_t)b->n_obs * 2));
+  PXR_TRY(b->project(b->cur, jac != 0, dxy.p));
+  if (uv) PXR_CUDA(cudaMemcpyAsync(uv, b->uv.p, (size_t)b->n_obs * 16, cudaMemcpyDeviceToHost, s));
+  if (xy) PXR_CUDA(cudaMemcpyAsync(xy, dxy.p, (size_t)b->n_obs * 16, cudaMemcpyDeviceToHost, s));
   PXR_CUDA(cudaStreamSynchronize(s));
   return PXR_OK;
 }

@@ -551,31 +551,26 @@ int BA::lm_iterate_block(int max_iteration) {
     PXR_TRY(compute_step_block(lm.radius));
     it.linear_solver_iterations = last_linear_iterations;
     PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 0, ctx->rank == 0 ? 1 : 0, interrupted);
-    PXR_TRY(apply_step(nullptr, nullptr));
+    PXR_TRY(apply_step());
     swap_sets();
-    const bool speculate = !lm.inner_enabled && !env.no_speculation;
+    // as in lm_iterate: with speculation the pass at the point the step moves to runs in Jacobian mode, and with inner
+    // iterations the trial cost comes from their round 0
+    const bool speculate = !env.no_speculation;
     const bool ran_inner = lm.inner_enabled;
-    int rc = project(1 - cur, speculate, nullptr);
-    if (rc == PXR_OK) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
+    const bool round0_cost = ran_inner && speculate;
+    // ceres skips inner iterations when the trial cost is not finite — a GLOBAL fact that is only known after the
+    // exchange; they are per-point and local, so they run regardless and their result is ignored in that case (the step
+    // is rejected)
+    int rc = round0_cost ? inner_iterations(1 - cur, scalars.p + 0) : project(1 - cur, speculate, nullptr);
+    if (rc == PXR_OK && !round0_cost) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
     if (rc != PXR_OK) { swap_sets(); return rc; }
     PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 1, ctx->rank == 0 ? 1 : 0, 0);
     if (ran_inner) {
-      // ceres skips them when the trial cost is not finite — a GLOBAL fact that is only known after the exchange; they are
-      // per-point and local, so they run regardless and their result is ignored in that case (the step is rejected)
-      rc = inner_iterations(1 - cur);
-      if (rc == PXR_OK) rc = project(1 - cur, false, nullptr);
-      if (rc == PXR_OK) rc = fm(0, nullptr, scalars.p + 0);
+      if (!round0_cost) rc = inner_iterations(1 - cur);
+      if (rc == PXR_OK) rc = project(1 - cur, speculate, nullptr);
+      if (rc == PXR_OK) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
+      if (rc == PXR_OK) rc = step_norm_between_sets();
       if (rc != PXR_OK) { swap_sets(); return rc; }
-      PXR_CUDA(cudaMemsetAsync(scalars.p + 11, 0, 16, s));
-      auto run = [&](const double* a, const double* b, int64_t n, double* acc) {
-        if (n <= 0) return;
-        PXR_LAUNCH(ctx, diff_norm_kernel, (unsigned)cdiv(n, 256), 256, 0, a, b, n, acc, deterministic ? det_scal_part.p : nullptr);
-        if (deterministic) PXR_LAUNCH(ctx, det_reduce_add_kernel, 1, 1024, 0, det_scal_part.p, cdiv(n, 256), 1, 0, acc);
-      };
-      run(cam[0].p, cam[1].p, (int64_t)n_cameras * kMaxK, scalars.p + 12);
-      run(q[0].p, q[1].p, (int64_t)n_images * 4, scalars.p + 12);
-      run(t[0].p, t[1].p, (int64_t)n_images * 3, scalars.p + 12);
-      run(X[0].p, X[1].p, n_points * 3, scalars.p + 11);
       PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 2, ctx->rank == 0 ? 1 : 0, 0);
     }
     PXR_TRY(exchange_scalars(11));

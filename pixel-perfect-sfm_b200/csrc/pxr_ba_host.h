@@ -234,10 +234,11 @@ struct BA {
   int evaluate(int set, bool jac, double* cost_out);
   int compute_step(double radius, bool* valid, double* model_cost_change);
   int chol_launch();
-  int apply_step(double* step_norm, double* x_norm);
+  int apply_step();
   int gradient_max_norm(double* out);
-  int inner_iterations(int set);
-  int inner_iterations_batched(int set);
+  // trial_cost (device scalar, optional): receives the cost at the starting point, reduced from round 0's records
+  int inner_iterations(int set, double* trial_cost = nullptr);
+  int inner_iterations_batched(int set, double* trial_cost);
   int eval_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev = nullptr, bool settle = true,
                 cudaEvent_t after_k0 = nullptr, cudaEvent_t after_k1 = nullptr, int64_t k0_bound = -1);
   int alloc_inner_jpt();                            // inner_jpt's one allocation: before the rounds, or a debug entry
@@ -247,7 +248,7 @@ struct BA {
   int capture_round_lists(const int64_t* plist, const int64_t* list, const unsigned long long* cnt);
   int capture_round_active();
   int project_point_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev, int64_t grid_bound);
-  int inner_rounds(int set);                       // the <= 52 rounds of inner_iterations_batched, without a host wait per round
+  int inner_rounds(int set, double* trial_cost);   // the <= 52 rounds of inner_iterations_batched, without a host wait per round
   unsigned long long* inner_cnt_host = nullptr;    // pinned, mapped [kInnerRounds][3]: each round's list lengths + the epoch of the call
   unsigned long long* inner_cnt_dev = nullptr;     // the same slots, device view (written by inner_step_kernel)
   unsigned long long inner_epoch = 0;              // incremented per inner_rounds call: tells this call's slots from stale ones
@@ -261,7 +262,7 @@ struct BA {
   DevBuf<unsigned long long> inner_counters;       // 3 x [observations, points], rotating
   DevBuf<double> inner_jpt;                        // [n_obs][6]: d(uv)/dX of the observations a round evaluated
   bool use_monolithic_inner = false;
-  int step_norm_between_sets(double* out);
+  int step_norm_between_sets();                    // enqueues the squared point / camera parts to scalars[11] / [12]
   int lm_begin();
   bool lm_finalize(int max_iteration);
   int lm_iterate(int max_iteration);

@@ -97,6 +97,13 @@ class BAHandle:
                                                         int(bool(count_on_device)), _p(uv), _p(jpt), _p(uv_full)))
         return dict(uv=uv, jpt=jpt, uv_full=uv_full)
 
+    def debug_project(self, jac):
+        """K0 over all observations, cost-only (jac False) or with Jacobians: uv [n_obs, 2] and xy [n_obs, 2]"""
+        n = self.problem.n_obs
+        uv, xy = np.empty((n, 2)), np.empty((n, 2))
+        _capi.check(self.lib.pxr_ba_debug_project(self.handle, int(bool(jac)), _p(uv), _p(xy)))
+        return dict(uv=uv, xy=xy)
+
     def debug_inner_capture(self, enable=True):
         """keep every round's lists in the batched inner iterations that follow (the host waits for every round)"""
         _capi.check(self.lib.pxr_ba_debug_inner_capture(self.handle, int(bool(enable))))
