@@ -1396,31 +1396,68 @@ int BA::gradient_max_norm(double* out) {
 }
 
 // -------------------------------------------------------------------------------- LM driver
-// Mirrors ceres::internal::TrustRegionMinimizer::Minimize (Ceres 2.1) with
-// LevenbergMarquardtStrategy, monotonic steps, Jacobi scaling, inner iterations.  The loop state
-// lives in the BA object so that a solve can be continued (pxr_ba_iterate) — bench.py times K
-// consecutive iterations of one trajectory after W warm-up iterations.
+// Mirrors ceres::internal::TrustRegionMinimizer::Minimize (Ceres 2.1) with LevenbergMarquardtStrategy, monotonic or
+// non-monotonic steps, Jacobi scaling, inner iterations; the rules themselves are TrustRegion's (pxr_lm.cuh).  The loop
+// state lives in the BA object so that a solve can be continued (pxr_ba_iterate) — bench.py times K consecutive
+// iterations of one trajectory after W warm-up iterations.  One loop serves both modes; lm_linearize_start, lm_trial
+// and lm_move hold what block mode (pxr_ba_block.cu) does differently: it enqueues a whole iteration and learns its
+// scalars from one exchange, where the single-GPU driver reads them back as it goes.
 int BA::lm_begin() {
-  if (block_mode) return lm_begin_block();
   PXR_CUDA(cudaSetDevice(ctx->device));
   lm = LMState();
-  lm.radius = opt.initial_trust_region_radius;
   lm.inner_enabled = opt.use_inner_iterations != 0;
   // ---- IterationZero
-  PXR_TRY(evaluate(cur, true, &lm.x_cost));
-  if (!std::isfinite(lm.x_cost)) return fail(PXR_ERR_NUMERIC, "initial cost is not finite");
-  if (nl > 0) PXR_LAUNCH(ctx, ba_scale_kernel, (unsigned)cdiv(nl, 256), 256, 0, diag.p, jscale.p, nl, opt.jacobi_scaling);
+  PXR_TRY(lm_linearize_start());
   std::memset(&lm.it, 0, sizeof(lm.it));
   lm.it.cost = lm.x_cost;
-  PXR_TRY(gradient_max_norm(&lm.it.gradient_max_norm));
+  PXR_TRY(lm_gradient(&lm.it.gradient_max_norm));
   lm.initial_cost = lm.minimum_cost = lm.x_cost;
-  lm.ev.init(lm.x_cost, opt.use_nonmonotonic_steps ? opt.max_consecutive_nonmonotonic_steps : 0);
+  TrustRegionOptions o;
+  o.max_consecutive_invalid_steps = opt.max_num_consecutive_invalid_steps;
+  o.max_nonmonotonic = opt.use_nonmonotonic_steps ? opt.max_consecutive_nonmonotonic_steps : 0;
+  o.initial_radius = opt.initial_trust_region_radius;
+  o.max_radius = opt.max_trust_region_radius;
+  o.min_radius = opt.min_trust_region_radius;
+  o.gradient_tolerance = opt.gradient_tolerance;
+  o.parameter_tolerance = opt.parameter_tolerance;
+  o.function_tolerance = opt.function_tolerance;
+  o.min_relative_decrease = opt.min_relative_decrease;
+  lm.tr.init(o, lm.x_cost);
   lm.best_is_current = true;
   lm.started = true;
   lm.pending_finalize = true;
   lm.term = 1;
   lm.message = "Maximum number of iterations reached.";
   return PXR_OK;
+}
+
+int BA::lm_linearize_start() {
+  if (!block_mode) {
+    PXR_TRY(evaluate(cur, true, &lm.x_cost));
+  } else {
+    PXR_TRY(project(cur, true, nullptr));
+    PXR_TRY(fm(1, nullptr, scalars.p + 0));
+    PXR_TRY(build_block());
+    PXR_TRY(global_cost_block(&lm.x_cost));
+  }
+  if (!std::isfinite(lm.x_cost)) return fail(PXR_ERR_NUMERIC, "initial cost is not finite");
+  if (!block_mode) {
+    if (nl > 0) PXR_LAUNCH(ctx, ba_scale_kernel, (unsigned)cdiv(nl, 256), 256, 0, diag.p, jscale.p, nl, opt.jacobi_scaling);
+  } else {
+    // block mode: point columns now, camera columns right after the first all-reduce (they need the global diagonal)
+    if (nl - nc > 0) PXR_LAUNCH(ctx, ba_scale_kernel, (unsigned)cdiv(nl - nc, 256), 256, 0, diag.p + nc, jscale.p + nc, nl - nc, opt.jacobi_scaling);
+    jscale_c_pending = true;
+  }
+  return PXR_OK;
+}
+
+int BA::lm_gradient(double* out) {
+  if (blk_lag_gmax) {   // block mode, several ranks: it arrives with the next all-reduce (finish_gmax_block at the end)
+    *out = std::numeric_limits<double>::quiet_NaN();
+    lm.gmax_pending = true;
+    return PXR_OK;
+  }
+  return gradient_max_norm(out);
 }
 
 // FinalizeIterationAndCheckIfMinimizerCanContinue
@@ -1433,65 +1470,37 @@ bool BA::lm_finalize(int max_iteration) {
       ++lm.n_succ;
       if (lm.x_cost < lm.minimum_cost) lm.minimum_cost = lm.x_cost;
     } else if (it.iteration > 0) ++lm.n_unsucc;
-    it.trust_region_radius = lm.radius;
+    it.trust_region_radius = lm.tr.radius;
     it.iteration_time_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - lm.it_start).count();
     lm.its.push_back(it);
     lm.pending_finalize = false;
   }
-  if (it.iteration >= max_iteration) { lm.term = 1; lm.message = "Maximum number of iterations reached."; return false; }
-  if (it.gradient_max_norm <= opt.gradient_tolerance) { lm.term = 0; lm.message = "Gradient tolerance reached."; lm.finished = true; return false; }
-  if (lm.radius < opt.min_trust_region_radius) { lm.term = 0; lm.message = "Minimum trust region radius reached."; lm.finished = true; return false; }
+  switch (lm.tr.stop(it.iteration, max_iteration, it.gradient_max_norm)) {
+    case TR_MAX_ITERATIONS: lm.term = 1; lm.message = "Maximum number of iterations reached."; return false;
+    case TR_GRADIENT_TOLERANCE: lm.term = 0; lm.message = "Gradient tolerance reached."; lm.finished = true; return false;
+    case TR_MIN_RADIUS: lm.term = 0; lm.message = "Minimum trust region radius reached."; lm.finished = true; return false;
+  }
   return true;
 }
 
-// Runs LM iterations until iteration index `max_iteration` (absolute) or termination.
-int BA::lm_iterate(int max_iteration) {
-  if (block_mode) return lm_iterate_block(max_iteration);
-  using clk = std::chrono::steady_clock;
-  if (!lm.started) PXR_TRY(lm_begin());
-  lm.it_start = clk::now();
-  while (!lm.finished && lm_finalize(max_iteration)) {
-    if (interrupt_pending()) {     // Ctrl-C in the host (util/src/py_interrupt.h:29-38): stop between iterations
-      lm.finished = true; lm.term = 3;
-      lm.message = "interrupted by the host";
-      return fail(PXR_ERR_INTERRUPTED, "interrupted by the host after LM iteration %d", lm.it.iteration);
-    }
-    lm.it_start = clk::now();
-    pxr_iteration_summary& it = lm.it;
-    const double prev_gmax = it.gradient_max_norm;
-    const int iteration = it.iteration + 1;
-    std::memset(&it, 0, sizeof(it));
-    it.iteration = iteration;
-    lm.pending_finalize = true;
-
-    bool valid = false;
-    double model_cost_change = 0;
-    PXR_TRY(compute_step(lm.radius, &valid, &model_cost_change));
-    it.linear_solver_iterations = last_linear_iterations;
-    it.step_is_valid = valid;
-    if (!valid) {
-      if (++lm.num_invalid >= opt.max_num_consecutive_invalid_steps) {
-        lm.term = 2; lm.finished = true;
-        lm.message = "Number of consecutive invalid steps more than Solver::Options::max_num_consecutive_invalid_steps";
-        break;
-      }
-      lm.radius /= lm.decrease_factor; lm.decrease_factor *= 2.0;
-      it.cost = lm.x_cost; it.gradient_max_norm = prev_gmax;
-      continue;
-    }
-    lm.num_invalid = 0;
-
-    // Trial point.  Ceres evaluates the cost here and, if the step is accepted, residuals AND Jacobians again at the
-    // point it moves to.  Both passes stream the same patch windows, so with speculation (DESIGN §4) the pass at that
-    // point runs in Jacobian mode right away, into the alternate buffer set; a rejected step merely discards it.
-    // Without inner iterations that pass is the trial pass.  With them the trial cost comes from inner-iteration round 0,
-    // which evaluates every observation at the trial point, and the pass after the rounds is the one at the final point.
-    // Ceres skips inner iterations when the trial cost is not finite; here they run regardless and their result is
-    // ignored (such a step is rejected, and its parameter set with it).  The costs and the norms of the step come back
-    // in one host round trip.  PXR_NO_SPECULATION: cost-only passes, and the accepted point is evaluated again.
-    const bool speculate = !env.no_speculation;
-    const bool ran_inner = lm.inner_enabled;
-    const bool round0_cost = ran_inner && speculate;
+// Enqueues the step and its trial evaluation, and reads back what the host decides on.
+int BA::lm_trial(bool interrupted, bool ran_inner, LMTrial* t) {
+  // Trial point.  Ceres evaluates the cost here and, if the step is accepted, residuals AND Jacobians again at the
+  // point it moves to.  Both passes stream the same patch windows, so with speculation (DESIGN §4) the pass at that
+  // point runs in Jacobian mode right away, into the alternate buffer set; a rejected step merely discards it.
+  // Without inner iterations that pass is the trial pass.  With them the trial cost comes from inner-iteration round 0,
+  // which evaluates every observation at the trial point, and the pass after the rounds is the one at the final point.
+  // Ceres skips inner iterations when the trial cost is not finite; here they run regardless and their result is
+  // ignored (such a step is rejected, and its parameter set with it).  PXR_NO_SPECULATION: cost-only passes, and the
+  // accepted point is evaluated again.
+  const bool speculate = !env.no_speculation;
+  const bool round0_cost = ran_inner && speculate;
+  if (!block_mode) {
+    // single GPU: an interrupt stops the solve before anything is enqueued
+    if (interrupted) { t->interrupted = true; return PXR_OK; }
+    // host synchronisation 1 of 2: the step's validity and model cost change
+    PXR_TRY(compute_step(lm.tr.radius, &t->valid, &t->model_cost_change));
+    if (!t->valid) return PXR_OK;     // single GPU: no trial after an invalid step
     PXR_TRY(apply_step());
     swap_sets();
     int rc = round0_cost ? inner_iterations(1 - cur, scalars.p + 0) : project(1 - cur, speculate, nullptr);
@@ -1506,56 +1515,170 @@ int BA::lm_iterate(int max_iteration) {
     if (rc == PXR_OK) rc = allreduce_f64(ctx, scalars.p + 0, ran_inner ? 2 : 1);
     double v[13] = {};     // [0] trial cost, [1] cost after the inner iterations, [5..8] apply_step's norms, [11..12] the step after them
     if (rc == PXR_OK) {
+      // host synchronisation 2 of 2: the costs and the norms of the step in one round trip
       cudaError_t e = cudaMemcpyAsync(v, scalars.p, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream);
       if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
       if (e != cudaSuccess) rc = fail(PXR_ERR_CUDA, "trial evaluation failed: %s", cudaGetErrorString(e));
     }
+    swap_sets();   // back: uv/obs_out/juv = linearisation at the current point again
+    PXR_TRY(rc);
+    t->cost = v[0]; t->inner_cost = v[1];
+    t->step_sq[0] = v[5]; t->step_sq[1] = v[7]; t->x_sq[0] = v[6]; t->x_sq[1] = v[8];
+    t->inner_step_sq[0] = v[11]; t->inner_step_sq[1] = v[12];
+    return PXR_OK;
+  }
+  // block mode: the whole iteration is enqueued before the host knows whether the step is valid, and the interrupt is
+  // agreed on through the scalar exchange (a rank must not leave alone)
+  cudaStream_t s = ctx->stream;
+  PXR_TRY(compute_step_block(lm.tr.radius));
+  pack_scalars(0, interrupted ? 1 : 0);
+  PXR_TRY(apply_step());
+  swap_sets();
+  // ceres skips inner iterations when the trial cost is not finite — a GLOBAL fact that is only known after the
+  // exchange; they are per-point and local, so they run regardless
+  int rc = round0_cost ? inner_iterations(1 - cur, scalars.p + 0) : project(1 - cur, speculate, nullptr);
+  if (rc == PXR_OK && !round0_cost) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
+  if (rc != PXR_OK) { swap_sets(); return rc; }
+  pack_scalars(1);
+  if (ran_inner) {
+    if (!round0_cost) rc = inner_iterations(1 - cur);
+    if (rc == PXR_OK) rc = project(1 - cur, speculate, nullptr);
+    if (rc == PXR_OK) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
+    if (rc == PXR_OK) rc = step_norm_between_sets();
     if (rc != PXR_OK) { swap_sets(); return rc; }
-    double candidate_cost = std::isfinite(v[0]) ? v[0] : std::numeric_limits<double>::max();
-    double step_norm = std::sqrt(v[5] + v[7]);
-    const double x_norm = std::sqrt(v[6] + v[8]);
-    const double next_cost = ran_inner ? v[1] : candidate_cost;     // the cost of the pass left in the alternate set
+    pack_scalars(2);
+  }
+  PXR_TRY(exchange_scalars(11));
+  double o[12]; double gmax_here = 0; int mfail = 0;
+  PXR_CUDA(cudaMemcpyAsync(o, mb_out.p, sizeof(o), cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaMemcpyAsync(&gmax_here, scalars.p + 10, 8, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaMemcpyAsync(&mfail, flags.p + 3, sizeof(int), cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));                         // the ONE host synchronisation of the iteration
+  swap_sets();   // back: uv/obs_out/juv = linearisation at the current point again
+  if (mfail) { lm.finished = true; lm.term = 2; return fail(PXR_ERR_NCCL, "a peer rank did not deliver its scalars (mailbox time-out)"); }
+  t->gmax = std::max(gmax_here, o[11]);    // camera part (global g_c) | point part (max over the ranks)
+  t->interrupted = o[10] > 0.0;
+  t->model_cost_change = -o[0];
+  t->valid = o[1] == 0.0 && std::isfinite(o[0]) && t->model_cost_change > 0.0;
+  t->cost = o[2]; t->inner_cost = o[7];
+  t->step_sq[0] = o[3]; t->step_sq[1] = o[5]; t->x_sq[0] = o[4]; t->x_sq[1] = o[6];
+  t->inner_step_sq[0] = o[8]; t->inner_step_sq[1] = o[9];
+  return PXR_OK;
+}
 
+// Moves the linearisation to the accepted point (cur already names it) and sets lm.x_cost and its max |g|.
+int BA::lm_move(double candidate_cost, double next_cost) {
+  pxr_iteration_summary& it = lm.it;
+  const bool reuse = !env.no_speculation && candidate_cost < std::numeric_limits<double>::max();
+  if (!block_mode) {
+    if (reuse) {
+      swap_sets();                   // the speculative pass IS the linearisation at the new point
+      PXR_TRY(build());
+      lm.x_cost = next_cost;         // single GPU: the cost of that pass
+    } else {
+      PXR_TRY(evaluate(cur, true, &lm.x_cost));
+    }
+  } else {
+    if (reuse) {
+      swap_sets();
+    } else {
+      PXR_TRY(project(cur, true, nullptr));
+      PXR_TRY(fm(1, nullptr, scalars.p + 0));
+    }
+    PXR_TRY(build_block());
+    lm.x_cost = candidate_cost;      // block mode: the trial cost (after the inner iterations) is the new cost
+  }
+  it.cost = lm.x_cost;
+  return lm_gradient(&it.gradient_max_norm);   // single GPU: a host synchronisation
+}
+
+// Runs LM iterations until iteration index `max_iteration` (absolute) or termination.
+int BA::lm_iterate(int max_iteration) {
+  using clk = std::chrono::steady_clock;
+  const double kMax = std::numeric_limits<double>::max();
+  if (!lm.started) PXR_TRY(lm_begin());
+  lm.it_start = clk::now();
+  while (!lm.finished && lm_finalize(max_iteration)) {
+    const bool interrupted = interrupt_pending();     // Ctrl-C in the host (util/src/py_interrupt.h:29-38)
+    lm.it_start = clk::now();
+    pxr_iteration_summary& it = lm.it;
+    const pxr_iteration_summary prev_it = it;
+    const double prev_gmax = it.gradient_max_norm;
+    const int iteration = it.iteration + 1;
+    std::memset(&it, 0, sizeof(it));
+    it.iteration = iteration;
+    lm.pending_finalize = true;
+
+    const bool ran_inner = lm.inner_enabled;
+    LMTrial t;
+    PXR_TRY(lm_trial(interrupted, ran_inner, &t));
+    it.linear_solver_iterations = last_linear_iterations;
+    if (lm.gmax_pending) {
+      // block mode, several ranks: max |g| at the CURRENT point arrives with this iteration's all-reduce; ceres tests it
+      // before starting the iteration: when it already meets the tolerance, this iteration never happened
+      lm.gmax_pending = false;
+      if (!lm.its.empty()) lm.its.back().gradient_max_norm = t.gmax;
+      if (t.gmax <= opt.gradient_tolerance) {
+        it = prev_it; it.gradient_max_norm = t.gmax;
+        lm.pending_finalize = false;
+        lm.term = 0; lm.message = "Gradient tolerance reached."; lm.finished = true;
+        break;
+      }
+    }
+    // the max |g| an invalid or rejected step reports: the one at the current point, which block mode with several
+    // ranks learns only now
+    const double known_gmax = blk_lag_gmax ? t.gmax : prev_gmax;
+    if (t.interrupted) {     // stop between iterations: this one never happened
+      it = prev_it; lm.pending_finalize = false;
+      lm.finished = true; lm.term = 3; lm.message = "interrupted by the host";
+      return fail(PXR_ERR_INTERRUPTED, "interrupted by the host after LM iteration %d", it.iteration);
+    }
+    it.step_is_valid = t.valid;
+    if (!t.valid) {
+      if (lm.tr.invalid_step()) {
+        lm.term = 2; lm.finished = true;
+        lm.message = "Number of consecutive invalid steps more than Solver::Options::max_num_consecutive_invalid_steps";
+        break;
+      }
+      it.cost = lm.x_cost; it.gradient_max_norm = known_gmax;
+      continue;
+    }
+    lm.tr.num_invalid = 0;
+
+    double model_cost_change = t.model_cost_change;
+    double candidate_cost = std::isfinite(t.cost) ? t.cost : kMax;
+    double step_norm = std::sqrt(t.step_sq[0] + t.step_sq[1]);
+    const double x_norm = std::sqrt(t.x_sq[0] + t.x_sq[1]);
+    const double next_cost = ran_inner ? t.inner_cost : candidate_cost;     // the cost of the pass left in the alternate set
     bool inner_useful = false;
-    if (ran_inner && candidate_cost < std::numeric_limits<double>::max()) {
+    if (ran_inner && candidate_cost < kMax) {
       ++lm.n_inner;
-      const double inner_cost = v[1];
+      const double inner_cost = t.inner_cost;
       if (std::isfinite(inner_cost)) {
         model_cost_change += candidate_cost - inner_cost;
         inner_useful = inner_cost < lm.x_cost;
         const double rel = 1.0 - inner_cost / candidate_cost;
         lm.inner_enabled = rel > opt.inner_iteration_tolerance;
         candidate_cost = inner_cost;
-        step_norm = std::sqrt(v[11] + v[12]);
+        step_norm = std::sqrt(t.inner_step_sq[0] + t.inner_step_sq[1]);
       }
     }
-    swap_sets();   // back: uv/obs_out/juv = linearisation at the current point again
     it.step_norm = step_norm;
-    if (step_norm <= opt.parameter_tolerance * (x_norm + opt.parameter_tolerance)) {
-      lm.term = 0; lm.message = "Parameter tolerance reached."; lm.finished = true; break;
-    }
     it.cost_change = lm.x_cost - candidate_cost;
-    if (std::fabs(it.cost_change) <= opt.function_tolerance * lm.x_cost) {
-      lm.term = 0; lm.message = "Function tolerance reached."; lm.finished = true; break;
+    const int tol = lm.tr.tolerance(step_norm, x_norm, it.cost_change, lm.x_cost);
+    if (tol) {
+      lm.term = 0; lm.finished = true;
+      lm.message = tol == TR_PARAMETER_TOLERANCE ? "Parameter tolerance reached." : "Function tolerance reached.";
+      break;
     }
-    it.relative_decrease = lm.ev.quality(candidate_cost, model_cost_change);
-    const bool ok = inner_useful || it.relative_decrease > opt.min_relative_decrease;
-    if (ok) {
+    it.relative_decrease = lm.tr.ev.quality(candidate_cost, model_cost_change);
+    if (inner_useful || lm.tr.successful(it.relative_decrease)) {
       cur = 1 - cur;
-      if (speculate && candidate_cost < std::numeric_limits<double>::max()) {
-        swap_sets();                 // the speculative pass IS the linearisation at the new point
-        PXR_TRY(build());
-        lm.x_cost = next_cost;
-      } else {
-        PXR_TRY(evaluate(cur, true, &lm.x_cost));
-      }
-      it.cost = lm.x_cost;
-      PXR_TRY(gradient_max_norm(&it.gradient_max_norm));
+      // The accepted cost: the single-GPU driver takes the post-inner pass (next_cost), block mode the trial cost after
+      // the inner iterations.  They differ only when the post-inner cost is not finite while the trial cost is.
+      PXR_TRY(lm_move(candidate_cost, next_cost));
       it.step_is_successful = 1;
-      lm.radius = lm.radius / std::max(1.0 / 3.0, 1.0 - std::pow(2.0 * it.relative_decrease - 1.0, 3));
-      lm.radius = std::min(opt.max_trust_region_radius, lm.radius);
-      lm.decrease_factor = 2.0;
-      lm.ev.accepted(candidate_cost, model_cost_change);
+      lm.tr.accept(it.relative_decrease, candidate_cost, model_cost_change);
       if (opt.use_nonmonotonic_steps) {
         // ceres copies x into the user's parameter blocks only when it is the best iterate so far
         // (FinalizeIterationAndCheckIfMinimizerCanContinue); a non-monotonic acceptance moves away from it, so the
@@ -1566,11 +1689,12 @@ int BA::lm_iterate(int max_iteration) {
     } else {
       it.step_is_successful = 0;
       it.cost = candidate_cost;
-      it.gradient_max_norm = prev_gmax;
-      lm.radius /= lm.decrease_factor; lm.decrease_factor *= 2.0;
+      it.gradient_max_norm = known_gmax;
+      lm.tr.reject();
     }
   }
   if (lm.x_cost < lm.minimum_cost) lm.minimum_cost = lm.x_cost;
+  if (lm.finished) PXR_TRY(finish_gmax_block());   // block mode, several ranks: the max |g| no iteration delivered
   PXR_CUDA(cudaStreamSynchronize(ctx->stream));
   return PXR_OK;
 }

@@ -2,10 +2,10 @@
 // packed reduced-camera blocks per LM iteration, a deterministic replicated solve, and the accept/reject scalars
 // exchanged through peer mailboxes over NVLink (pxr_api.cu).  Layout and invariants: pxr_block.cuh.
 //
-// Same trust-region logic as BA::lm_iterate (ceres TrustRegionMinimizer 2.1, reference call site
-// bundle_adjustment/src/bundle_optimizer.h:224); what differs is WHEN the host learns the scalars: every LM iteration
-// enqueues  assemble -> all-reduce -> solve -> back-substitute -> plus -> trial evaluation (-> inner iterations)
-// without looking at anything, then exchanges all partial sums at once and synchronises ONCE.
+// BA::lm_iterate (pxr_ba.cu) drives it with the same trust-region rules as one GPU; what differs is WHEN the host learns
+// the scalars: every LM iteration enqueues  assemble -> all-reduce -> solve -> back-substitute -> plus -> trial
+// evaluation (-> inner iterations)  without looking at anything, then exchanges all partial sums at once and
+// synchronises ONCE.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -89,6 +89,10 @@ SparseSchur BA::sparse_blk(bool global) {
   q.key_a = ss_key_a.p; q.key_b = ss_key_b.p; q.key_self = ss_key_self.p;
   q.Himg = pk(global); q.Bk = pk(global) + pk_off_B;
   return q;
+}
+
+void BA::pack_scalars(int stage, int interrupted) {
+  PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, stage, ctx->rank == 0 ? 1 : 0, interrupted);
 }
 
 // mb_in[0 .. n_sum) are summed over the ranks, mb_in[11] is maximised; results in mb_out (same slots)
@@ -426,7 +430,7 @@ int BA::compute_step_block(double radius) {
 int BA::global_cost_block(double* cost_out) {
   cudaStream_t s = ctx->stream;
   PXR_CUDA(cudaMemsetAsync(flags.p + 3, 0, sizeof(int), s));
-  PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 3, ctx->rank == 0 ? 1 : 0, 0);
+  pack_scalars(3);
   PXR_TRY(exchange_scalars(1));
   double c = 0; int mfail = 0;
   PXR_CUDA(cudaMemcpyAsync(&c, mb_out.p, 8, cudaMemcpyDeviceToHost, s));
@@ -440,7 +444,7 @@ int BA::global_cost_block(double* cost_out) {
 int BA::compute_step_block_sync(double radius, bool* valid, double* model_cost_change) {
   cudaStream_t s = ctx->stream;
   PXR_TRY(compute_step_block(radius));
-  PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 0, ctx->rank == 0 ? 1 : 0, 0);
+  pack_scalars(0);
   PXR_TRY(exchange_scalars(2));
   double o[2] = {0, 0}; int mfail = 0;
   PXR_CUDA(cudaMemcpyAsync(o, mb_out.p, 16, cudaMemcpyDeviceToHost, s));
@@ -475,36 +479,6 @@ int BA::pcg_solve_block() {
   return run_cg(spmv);
 }
 
-// -------------------------------------------------------------------------------- LM driver (block mode)
-int BA::lm_begin_block() {
-  PXR_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->stream;
-  lm = LMState();
-  lm.radius = opt.initial_trust_region_radius;
-  lm.inner_enabled = opt.use_inner_iterations != 0;
-  // ---- IterationZero
-  PXR_TRY(project(cur, true, nullptr));
-  PXR_TRY(fm(1, nullptr, scalars.p + 0));
-  PXR_TRY(build_block());
-  PXR_TRY(global_cost_block(&lm.x_cost));
-  if (!std::isfinite(lm.x_cost)) return fail(PXR_ERR_NUMERIC, "initial cost is not finite");
-  // Jacobi scaling: point columns now, camera columns right after the first all-reduce (they need the global diagonal)
-  if (nl - nc > 0) PXR_LAUNCH(ctx, ba_scale_kernel, (unsigned)cdiv(nl - nc, 256), 256, 0, diag.p + nc, jscale.p + nc, nl - nc, opt.jacobi_scaling);
-  jscale_c_pending = true;
-  std::memset(&lm.it, 0, sizeof(lm.it));
-  lm.it.cost = lm.x_cost;
-  if (blk_lag_gmax) { lm.it.gradient_max_norm = std::numeric_limits<double>::quiet_NaN(); lm.gmax_pending = true; }
-  else { PXR_TRY(gradient_max_norm(&lm.it.gradient_max_norm)); lm.gmax_pending = false; }
-  lm.initial_cost = lm.minimum_cost = lm.x_cost;
-  lm.ev.init(lm.x_cost, opt.use_nonmonotonic_steps ? opt.max_consecutive_nonmonotonic_steps : 0);
-  lm.best_is_current = true;
-  lm.started = true;
-  lm.pending_finalize = true;
-  lm.term = 1;
-  lm.message = "Maximum number of iterations reached.";
-  return PXR_OK;
-}
-
 // max |g| of the current point when no further LM iteration will deliver it: one small all-reduce of g_c, and the
 // per-rank point maxima through the scalar exchange
 int BA::finish_gmax_block() {
@@ -517,7 +491,7 @@ int BA::finish_gmax_block() {
     PXR_LAUNCH(ctx, ba_gradmax_kernel, (unsigned)cdiv(n, 256), 256, 0, dev(), pk(true) + pk_off_gc, q[cur].p, 0, scalars.p + 10);
   }
   PXR_CUDA(cudaMemsetAsync(flags.p + 3, 0, sizeof(int), s));
-  PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 3, ctx->rank == 0 ? 1 : 0, 0);
+  pack_scalars(3);
   PXR_TRY(exchange_scalars(1));
   double gcm = 0, gpm = 0;
   PXR_CUDA(cudaMemcpyAsync(&gcm, scalars.p + 10, 8, cudaMemcpyDeviceToHost, s));
@@ -527,155 +501,6 @@ int BA::finish_gmax_block() {
   lm.it.gradient_max_norm = g;
   if (!lm.its.empty() && !(lm.its.back().gradient_max_norm == lm.its.back().gradient_max_norm)) lm.its.back().gradient_max_norm = g;
   lm.gmax_pending = false;
-  return PXR_OK;
-}
-
-int BA::lm_iterate_block(int max_iteration) {
-  using clk = std::chrono::steady_clock;
-  cudaStream_t s = ctx->stream;
-  if (!lm.started) PXR_TRY(lm_begin_block());
-  lm.it_start = clk::now();
-  const double kMax = std::numeric_limits<double>::max();
-  while (!lm.finished && lm_finalize(max_iteration)) {
-    const int interrupted = interrupt_pending() ? 1 : 0;      // agreed on through the scalar exchange (a rank must not leave alone)
-    lm.it_start = clk::now();
-    pxr_iteration_summary& it = lm.it;
-    const pxr_iteration_summary prev_it = it;
-    const double prev_gmax = it.gradient_max_norm;
-    const int iteration = it.iteration + 1;
-    std::memset(&it, 0, sizeof(it));
-    it.iteration = iteration;
-    lm.pending_finalize = true;
-
-    // ---- enqueue the whole iteration
-    PXR_TRY(compute_step_block(lm.radius));
-    it.linear_solver_iterations = last_linear_iterations;
-    PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 0, ctx->rank == 0 ? 1 : 0, interrupted);
-    PXR_TRY(apply_step());
-    swap_sets();
-    // as in lm_iterate: with speculation the pass at the point the step moves to runs in Jacobian mode, and with inner
-    // iterations the trial cost comes from their round 0
-    const bool speculate = !env.no_speculation;
-    const bool ran_inner = lm.inner_enabled;
-    const bool round0_cost = ran_inner && speculate;
-    // ceres skips inner iterations when the trial cost is not finite — a GLOBAL fact that is only known after the
-    // exchange; they are per-point and local, so they run regardless and their result is ignored in that case (the step
-    // is rejected)
-    int rc = round0_cost ? inner_iterations(1 - cur, scalars.p + 0) : project(1 - cur, speculate, nullptr);
-    if (rc == PXR_OK && !round0_cost) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
-    if (rc != PXR_OK) { swap_sets(); return rc; }
-    PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 1, ctx->rank == 0 ? 1 : 0, 0);
-    if (ran_inner) {
-      if (!round0_cost) rc = inner_iterations(1 - cur);
-      if (rc == PXR_OK) rc = project(1 - cur, speculate, nullptr);
-      if (rc == PXR_OK) rc = fm(speculate ? 1 : 0, nullptr, scalars.p + 0);
-      if (rc == PXR_OK) rc = step_norm_between_sets();
-      if (rc != PXR_OK) { swap_sets(); return rc; }
-      PXR_LAUNCH(ctx, blk_pack_scalars_kernel, 1, 1, 0, scalars.p, flags.p, mb_in.p, 2, ctx->rank == 0 ? 1 : 0, 0);
-    }
-    PXR_TRY(exchange_scalars(11));
-    double o[12]; double gmax_here = 0; int mfail = 0;
-    PXR_CUDA(cudaMemcpyAsync(o, mb_out.p, sizeof(o), cudaMemcpyDeviceToHost, s));
-    PXR_CUDA(cudaMemcpyAsync(&gmax_here, scalars.p + 10, 8, cudaMemcpyDeviceToHost, s));
-    PXR_CUDA(cudaMemcpyAsync(&mfail, flags.p + 3, sizeof(int), cudaMemcpyDeviceToHost, s));
-    PXR_CUDA(cudaStreamSynchronize(s));                         // the ONE host synchronisation of the iteration
-    swap_sets();   // back: uv/obs_out/juv = linearisation at the current point again
-    if (mfail) { lm.finished = true; lm.term = 2; return fail(PXR_ERR_NCCL, "a peer rank did not deliver its scalars (mailbox time-out)"); }
-    gmax_here = std::max(gmax_here, o[11]);    // camera part (global g_c) | point part (max over the ranks)
-
-    // ---- what the host would have known earlier on one GPU
-    if (lm.gmax_pending) {
-      // max |g| at the CURRENT point arrives with this iteration's all-reduce; ceres tests it before starting the
-      // iteration: when it already meets the tolerance, this iteration never happened
-      lm.gmax_pending = false;
-      if (!lm.its.empty()) lm.its.back().gradient_max_norm = gmax_here;
-      if (gmax_here <= opt.gradient_tolerance) {
-        it = prev_it; it.gradient_max_norm = gmax_here;
-        lm.pending_finalize = false;
-        lm.term = 0; lm.message = "Gradient tolerance reached."; lm.finished = true;
-        break;
-      }
-    }
-    const double known_gmax = blk_lag_gmax ? gmax_here : prev_gmax;
-    if (o[10] > 0.0) {
-      it = prev_it; lm.pending_finalize = false;
-      lm.finished = true; lm.term = 3; lm.message = "interrupted by the host";
-      return fail(PXR_ERR_INTERRUPTED, "interrupted by the host after LM iteration %d", it.iteration);
-    }
-    double model_cost_change = -o[0];
-    const bool valid = o[1] == 0.0 && std::isfinite(o[0]) && model_cost_change > 0.0;
-    it.step_is_valid = valid;
-    if (!valid) {
-      if (++lm.num_invalid >= opt.max_num_consecutive_invalid_steps) {
-        lm.term = 2; lm.finished = true;
-        lm.message = "Number of consecutive invalid steps more than Solver::Options::max_num_consecutive_invalid_steps";
-        break;
-      }
-      lm.radius /= lm.decrease_factor; lm.decrease_factor *= 2.0;
-      it.cost = lm.x_cost; it.gradient_max_norm = known_gmax;
-      continue;
-    }
-    lm.num_invalid = 0;
-    double candidate_cost = o[2];
-    if (!std::isfinite(candidate_cost)) candidate_cost = kMax;
-    double step_norm = std::sqrt(o[3] + o[5]);
-    const double x_norm = std::sqrt(o[4] + o[6]);
-    bool inner_useful = false;
-    if (ran_inner && candidate_cost < kMax) {
-      ++lm.n_inner;
-      const double inner_cost = o[7];
-      if (std::isfinite(inner_cost)) {
-        model_cost_change += candidate_cost - inner_cost;
-        inner_useful = inner_cost < lm.x_cost;
-        const double rel = 1.0 - inner_cost / candidate_cost;
-        lm.inner_enabled = rel > opt.inner_iteration_tolerance;
-        candidate_cost = inner_cost;
-        step_norm = std::sqrt(o[8] + o[9]);
-      }
-    }
-    it.step_norm = step_norm;
-    if (step_norm <= opt.parameter_tolerance * (x_norm + opt.parameter_tolerance)) {
-      lm.term = 0; lm.message = "Parameter tolerance reached."; lm.finished = true; break;
-    }
-    it.cost_change = lm.x_cost - candidate_cost;
-    if (std::fabs(it.cost_change) <= opt.function_tolerance * lm.x_cost) {
-      lm.term = 0; lm.message = "Function tolerance reached."; lm.finished = true; break;
-    }
-    it.relative_decrease = lm.ev.quality(candidate_cost, model_cost_change);
-    const bool ok = inner_useful || it.relative_decrease > opt.min_relative_decrease;
-    if (ok) {
-      cur = 1 - cur;
-      if (speculate && candidate_cost < kMax) {
-        swap_sets();                 // the speculative pass IS the linearisation at the new point
-        PXR_TRY(build_block());
-      } else {
-        PXR_TRY(project(cur, true, nullptr));
-        PXR_TRY(fm(1, nullptr, scalars.p + 0));
-        PXR_TRY(build_block());
-      }
-      lm.x_cost = candidate_cost;    // same point, same residuals: the trial cost is the new cost
-      it.cost = lm.x_cost;
-      if (blk_lag_gmax) { it.gradient_max_norm = std::numeric_limits<double>::quiet_NaN(); lm.gmax_pending = true; }
-      else PXR_TRY(gradient_max_norm(&it.gradient_max_norm));
-      it.step_is_successful = 1;
-      lm.radius = lm.radius / std::max(1.0 / 3.0, 1.0 - std::pow(2.0 * it.relative_decrease - 1.0, 3));
-      lm.radius = std::min(opt.max_trust_region_radius, lm.radius);
-      lm.decrease_factor = 2.0;
-      lm.ev.accepted(candidate_cost, model_cost_change);
-      if (opt.use_nonmonotonic_steps) {
-        if (lm.x_cost < lm.minimum_cost) lm.best_is_current = true;
-        else if (lm.best_is_current) { PXR_TRY(save_best(1 - cur)); lm.best_is_current = false; }
-      }
-    } else {
-      it.step_is_successful = 0;
-      it.cost = candidate_cost;
-      it.gradient_max_norm = known_gmax;
-      lm.radius /= lm.decrease_factor; lm.decrease_factor *= 2.0;
-    }
-  }
-  if (lm.x_cost < lm.minimum_cost) lm.minimum_cost = lm.x_cost;
-  if (lm.finished) PXR_TRY(finish_gmax_block());
-  PXR_CUDA(cudaStreamSynchronize(s));
   return PXR_OK;
 }
 

@@ -18,6 +18,7 @@
 #include "pxr_geo.cuh"
 #include "pxr_inner.cuh"
 #include "pxr_internal.h"
+#include "pxr_lm.cuh"
 #include "pxr_pcg.cuh"
 #include "pxr_sparse_schur.cuh"
 #include "pxr_block.cuh"
@@ -29,36 +30,27 @@ int fm_max_partials(pxr_ctx* ctx);
 int launch_fm_eval(pxr_ctx* ctx, int dtype, int C, int mode, bool float_simd, const FmEvalArgs& a, int* n_partials);
 int launch_inner(pxr_ctx* ctx, int dtype, int C, bool float_simd, const InnerArgs& a);
 
-// ceres::internal::TrustRegionStepEvaluator (Conn, Gould & Toint, algorithm 10.1.2); max_nonmonotonic == 0 is the
-// monotonic minimizer.  Same arithmetic as oracle/orc_trust_region.h::StepEvaluator.
-struct StepEvaluator {
-  int max_nonmonotonic = 0, num_consecutive_nonmonotonic_steps = 0;
-  double minimum_cost = 0, current_cost = 0, reference_cost = 0, candidate_cost = 0;
-  double acc_reference = 0, acc_candidate = 0;
-  void init(double c, int max_nm) { *this = StepEvaluator(); max_nonmonotonic = max_nm; minimum_cost = current_cost = reference_cost = candidate_cost = c; }
-  double quality(double cost, double mcc) const {
-    if (cost >= std::numeric_limits<double>::max()) return std::numeric_limits<double>::lowest();
-    return std::max((current_cost - cost) / mcc, (reference_cost - cost) / (acc_reference + mcc));
-  }
-  void accepted(double cost, double mcc) {
-    current_cost = cost; acc_candidate += mcc; acc_reference += mcc;
-    if (current_cost < minimum_cost) { minimum_cost = current_cost; num_consecutive_nonmonotonic_steps = 0; candidate_cost = current_cost; acc_candidate = 0; }
-    else { ++num_consecutive_nonmonotonic_steps; if (current_cost > candidate_cost) { candidate_cost = current_cost; acc_candidate = 0; } }
-    if (num_consecutive_nonmonotonic_steps == max_nonmonotonic) { reference_cost = candidate_cost; acc_reference = acc_candidate; }
-  }
-};
-
 struct LMState {
   bool started = false, finished = false, pending_finalize = false, inner_enabled = false;
-  StepEvaluator ev;
+  TrustRegion tr;
   bool gmax_pending = false;       // block mode, several ranks: max |g| of the current point arrives with the next all-reduce
   bool best_is_current = true;     // non-monotonic steps: the lowest-cost iterate lives in BA::best_* when false
-  double x_cost = 0, radius = 1e4, decrease_factor = 2.0, initial_cost = 0, minimum_cost = 0;
-  int num_invalid = 0, n_succ = 0, n_unsucc = 0, n_inner = 0, term = 1;
+  double x_cost = 0, initial_cost = 0, minimum_cost = 0;
+  int n_succ = 0, n_unsucc = 0, n_inner = 0, term = 1;
   pxr_iteration_summary it;
   std::vector<pxr_iteration_summary> its;
   std::string message;
   std::chrono::steady_clock::time_point it_start;
+};
+
+// What the host learns about one LM step: BA::lm_trial's read-back
+struct LMTrial {
+  bool interrupted = false, valid = false;
+  double model_cost_change = 0;
+  double cost = 0, inner_cost = 0;                 // the trial cost, and the cost after the inner iterations
+  double step_sq[2] = {}, x_sq[2] = {};            // squared camera / point parts of |step| and |x|
+  double inner_step_sq[2] = {};                    // the same parts of the step after the inner iterations
+  double gmax = 0;                                 // block mode: max |g| at the current point, from the exchange
 };
 
 struct BA {
@@ -163,9 +155,8 @@ struct BA {
   int compute_step_block_sync(double radius, bool* valid, double* model_cost_change);   // + exchange + read-back (debug entry points)
   int global_cost_block(double* cost_out);         // scalars[0] summed over the ranks
   int pcg_solve_block();
-  int lm_begin_block();
-  int lm_iterate_block(int max_iteration);
   int finish_gmax_block();
+  void pack_scalars(int stage, int interrupted = 0);   // blk_pack_scalars_kernel: this rank's scalars -> mb_in
   int exchange_scalars(int n_sum);                 // mb_in -> mb_out (peer mailboxes, or NCCL when they are unavailable)
   std::vector<int32_t> h_chunk_key_local;
   std::vector<int64_t> h_key_code_local;           // local key codes in build order (set by build_schur_pairs)
@@ -263,9 +254,14 @@ struct BA {
   DevBuf<double> inner_jpt;                        // [n_obs][6]: d(uv)/dX of the observations a round evaluated
   bool use_monolithic_inner = false;
   int step_norm_between_sets();                    // enqueues the squared point / camera parts to scalars[11] / [12]
+  // LM driver (pxr_ba.cu), one loop for both modes; the three lm_* steps below are what differs with block_mode
   int lm_begin();
   bool lm_finalize(int max_iteration);
   int lm_iterate(int max_iteration);
+  int lm_linearize_start();                         // IterationZero's evaluation, cost and Jacobi scaling
+  int lm_trial(bool interrupted, bool ran_inner, LMTrial* t);   // enqueue the step and its trial, read back t
+  int lm_move(double candidate_cost, double next_cost);          // linearise at the accepted point: x_cost, |g|
+  int lm_gradient(double* out);                     // max |g| now, or NaN with lm.gmax_pending
   void fill_summary(pxr_summary* sum, double seconds, int64_t launches);
   int solve(pxr_summary* sum);
   int read_params(double* cam_o, double* q_o, double* t_o, double* X_o);

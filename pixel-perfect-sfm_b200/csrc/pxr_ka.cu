@@ -428,16 +428,21 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
   }
   __syncthreads();
   int iter = 0, invalid = 0, n_succ = 0, n_unsucc = 0, term = 1;
-  // ceres TrustRegionStepEvaluator (uniform over the CTA: every input is a block-wide reduction)
-  DevStepEvaluator ev;
+  // the trust-region rules of pxr_lm.cuh: thread 0 keeps radius and decrease factor in the C_RADIUS / C_DECF slots (a
+  // per-thread copy costs registers); every input of the decisions is a block-wide reduction, so each thread takes them,
+  // counts invalid steps and holds a step evaluator itself
+  const TrustRegionOptions o = {a.max_invalid, a.max_nonmonotonic, a.radius0, a.max_radius, a.min_radius, a.gtol, a.ptol,
+                                a.ftol, a.min_rel_dec};
+  StepEvaluator ev;
   ev.init(x_cost, a.max_nonmonotonic);
   double minimum_cost = x_cost;     // ceres keeps the lowest-cost iterate in the user's parameter blocks
   while (true) {
     // FinalizeIterationAndCheckIfMinimizerCanContinue
     if (w.ctrl[C_STOP] != 0.0) { term = 2; break; }
-    if (iter >= a.max_iter) { term = 1; break; }
-    if (w.ctrl[C_GMAX] <= a.gtol) { term = 0; break; }
-    if (w.ctrl[C_RADIUS] < a.min_radius) { term = 0; break; }
+    if (const int stop = tr_stop(o, w.ctrl[C_RADIUS], iter, a.max_iter, w.ctrl[C_GMAX])) {
+      term = stop == TR_MAX_ITERATIONS ? 1 : 0;
+      break;
+    }
     ++iter;
     const double radius = w.ctrl[C_RADIUS];
     // ---- LM step: (H + D) delta = -g
@@ -495,9 +500,9 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
     }
     }
     if (!valid) {
-      if (++invalid >= a.max_invalid) { term = 2; break; }
+      if (tr_invalid_stop(o, invalid)) { term = 2; break; }
       __syncthreads();
-      if (tid == 0) { w.ctrl[C_RADIUS] /= w.ctrl[C_DECF]; w.ctrl[C_DECF] *= 2.0; }
+      if (tid == 0) tr_reject(w.ctrl[C_RADIUS], w.ctrl[C_DECF]);
       __syncthreads();
       continue;
     }
@@ -562,10 +567,9 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
     }
     // ---- tolerances and step acceptance
     double sn = 0; { double v = 0; for (int i = tid; i < n; i += kKAThreads) { const double d = w.x[i] - w.cand[i]; v += d * d; } sn = sqrt(block_sum(v)); }
-    if (sn <= a.ptol * (w.ctrl[C_XNORM] + a.ptol)) { term = 0; break; }            // parameter tolerance: step not applied
-    if (fabs(x_cost - candidate_cost) <= a.ftol * x_cost) { term = 0; break; }     // function tolerance: step not applied
+    if (tr_tolerance(o, sn, w.ctrl[C_XNORM], x_cost - candidate_cost, x_cost)) { term = 0; break; }   // step not applied
     const double rel = ev.quality(candidate_cost, mcc);
-    if (rel > a.min_rel_dec) {
+    if (tr_successful(o, rel)) {
       __syncthreads();
       for (int i = tid; i < n; i += kKAThreads) w.x[i] = w.cand[i];
       x_cost = ka_evaluate<T, C, FS, REF>(a, w, eb, ee, n, w.x, 2, w.g);
@@ -573,9 +577,8 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
       reduce_max_proj_grad();
       if (tid == 0) {
         w.ctrl[C_GMAX] = w.ctrl[C_TMP];
-        double r2 = w.ctrl[C_RADIUS] / fmax(1.0 / 3.0, 1.0 - pow(2.0 * rel - 1.0, 3.0));
-        w.ctrl[C_RADIUS] = fmin(a.max_radius, r2);
-        w.ctrl[C_DECF] = 2.0; w.ctrl[C_XCOST] = x_cost;
+        tr_accept(o, w.ctrl[C_RADIUS], w.ctrl[C_DECF], rel);
+        w.ctrl[C_XCOST] = x_cost;
       }
       ++n_succ;
       ev.accepted(candidate_cost, mcc);
@@ -585,7 +588,7 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
       }
     } else {
       __syncthreads();
-      if (tid == 0) { w.ctrl[C_RADIUS] /= w.ctrl[C_DECF]; w.ctrl[C_DECF] *= 2.0; }
+      if (tid == 0) tr_reject(w.ctrl[C_RADIUS], w.ctrl[C_DECF]);
       ++n_unsucc;
     }
     __syncthreads();

@@ -10,8 +10,8 @@
 //               per warp; the warps' partials are summed in warp order, so a query's bits never depend on its neighbours
 //   LM          BA::lm_begin / lm_iterate (pxr_ba.cu) for one free image, no free points, no inner iterations: Jacobi
 //               scaling from iteration zero, clamped LM diagonal, invalid steps, parameter / function / gradient
-//               tolerances, ceres' step evaluator (pxr_lm.cuh) with use_nonmonotonic_steps and the lowest-cost iterate
-//               written back, the radius update and the termination types of lm_finalize
+//               tolerances, step quality and radius update through the trust-region rules of pxr_lm.cuh, with
+//               use_nonmonotonic_steps, the lowest-cost iterate written back and the termination types of lm_finalize
 //   solve       exact dense Cholesky of the damped n x n system (n = 6 + free intrinsics <= 18), one thread
 // The host packs consecutive queries into waves that fit a byte budget; one wave is one launch, and the next wave's
 // upload is enqueued before the host waits for the current one.
@@ -243,11 +243,11 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
   // ---- LM state: thread 0 takes every scalar decision, the CTA evaluates
   __shared__ double sL[kQTri], sd[kQMaxN], sscale[kQMaxN];
   const double initial_cost = x_cost;
-  double radius = a.radius0, decf = 2.0, min_cost = x_cost, mcc = 0.0, step_norm = 0.0, x_norm = 0.0, prev_gmax = 0.0;
-  int n_succ = 0, n_unsucc = 0, num_invalid = 0, term = 1, n_its = 0, cur = 0;
+  double min_cost = x_cost, mcc = 0.0, step_norm = 0.0, x_norm = 0.0, prev_gmax = 0.0;
+  int n_succ = 0, n_unsucc = 0, term = 1, n_its = 0, cur = 0;
   bool pending = true, best_is_current = true;
   pxr_iteration_summary it = pxr_iteration_summary();
-  DevStepEvaluator ev;
+  TrustRegion tr;
   double xn_points = 0.0;     // ||X||^2 of the constant points: part of ceres' ||x|| (ba_plus_kernel)
   if (tid == 0) {
     for (int i = 0; i < n; ++i) sscale[i] = a.jacobi_scaling ? 1.0 / (1.0 + sqrt(sH[0][qtri(i, i)])) : 1.0;
@@ -255,7 +255,8 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
       for (int k = 0; k < 3; ++k) { const double x = a.xyz[3 * o + k]; xn_points += x * x; }
     it.cost = x_cost;
     it.gradient_max_norm = qba_gradmax(sg[0], sx[0] + kMaxK, n);
-    ev.init(x_cost, a.max_nonmonotonic);
+    tr.init({a.max_invalid, a.max_nonmonotonic, a.radius0, a.max_radius, a.min_radius, a.gtol, a.ptol, a.ftol, a.min_rel_dec},
+            x_cost);
   }
   while (true) {
     if (tid == 0) {
@@ -264,14 +265,15 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
       if (pending) {
         if (it.step_is_successful) { ++n_succ; if (x_cost < min_cost) min_cost = x_cost; }
         else if (it.iteration > 0) ++n_unsucc;
-        it.trust_region_radius = radius;
+        it.trust_region_radius = tr.radius;
         if (a.iters && n_its < a.iter_cap) a.iters[(int64_t)q * a.iter_cap + n_its] = it;
         ++n_its;
         pending = false;
       }
-      if (it.iteration >= a.max_iter) { term = 1; action = QA_STOP; }
-      else if (it.gradient_max_norm <= a.gtol) { term = 0; action = QA_STOP; }
-      else if (radius < a.min_radius) { term = 0; action = QA_STOP; }
+      if (const int stop = tr.stop(it.iteration, a.max_iter, it.gradient_max_norm)) {
+        term = stop == TR_MAX_ITERATIONS ? 1 : 0;
+        action = QA_STOP;
+      }
       if (action != QA_STOP) {
         prev_gmax = it.gradient_max_norm;
         const int iteration = it.iteration + 1;
@@ -286,7 +288,7 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
         for (int i = 0; i < n * (n + 1) / 2; ++i) L[i] = H[i];
         for (int i = 0; i < n; ++i) {
           const double s2 = sscale[i] * sscale[i];
-          L[qtri(i, i)] += fmin(fmax(H[qtri(i, i)] * s2, a.min_diag), a.max_diag) / (radius * s2);
+          L[qtri(i, i)] += fmin(fmax(H[qtri(i, i)] * s2, a.min_diag), a.max_diag) / (tr.radius * s2);
         }
         bool ok = true;
         for (int j = 0; j < n && ok; ++j) {
@@ -325,14 +327,13 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
         it.linear_solver_iterations = 1;
         it.step_is_valid = valid;
         if (!valid) {
-          if (++num_invalid >= a.max_invalid) { term = 2; action = QA_STOP; }
+          if (tr.invalid_step()) { term = 2; action = QA_STOP; }
           else {
-            radius /= decf; decf *= 2.0;
             it.cost = x_cost; it.gradient_max_norm = prev_gmax;
             action = QA_SKIP;
           }
         } else {
-          num_invalid = 0;
+          tr.num_invalid = 0;
           // ---- candidate = Plus(x, delta) and the norms ba_plus_kernel forms (this image and its camera)
           const double* x = sx[0];
           double* xc = sx[1];
@@ -370,35 +371,29 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
       int act = QA_EVAL;
       if (!isfinite(candidate_cost)) candidate_cost = 1.7976931348623157e308;
       it.step_norm = step_norm;
-      if (step_norm <= a.ptol * (x_norm + a.ptol)) { term = 0; act = QA_STOP; }    // parameter tolerance: step not applied
+      it.cost_change = x_cost - candidate_cost;
+      if (tr.tolerance(step_norm, x_norm, it.cost_change, x_cost)) { term = 0; act = QA_STOP; }   // step not applied
       else {
-        it.cost_change = x_cost - candidate_cost;
-        if (fabs(it.cost_change) <= a.ftol * x_cost) { term = 0; act = QA_STOP; }  // function tolerance: step not applied
-        else {
-          it.relative_decrease = ev.quality(candidate_cost, mcc);
-          if (it.relative_decrease > a.min_rel_dec) {
-            if (a.max_nonmonotonic > 0 && !(candidate_cost < min_cost) && best_is_current) {
-              for (int i = 0; i < kQParams; ++i) sx[2][i] = sx[0][i];    // leaving the best iterate: keep it
-              best_is_current = false;
-            } else if (a.max_nonmonotonic > 0 && candidate_cost < min_cost) {
-              best_is_current = true;
-            }
-            for (int i = 0; i < kQParams; ++i) sx[0][i] = sx[1][i];
-            cur = 1 - cur;
-            x_cost = candidate_cost;
-            it.cost = x_cost;
-            it.gradient_max_norm = qba_gradmax(sg[cur], sx[0] + kMaxK, n);
-            it.step_is_successful = 1;
-            radius = radius / fmax(1.0 / 3.0, 1.0 - pow(2.0 * it.relative_decrease - 1.0, 3.0));
-            radius = fmin(a.max_radius, radius);
-            decf = 2.0;
-            ev.accepted(candidate_cost, mcc);
-          } else {
-            it.step_is_successful = 0;
-            it.cost = candidate_cost;
-            it.gradient_max_norm = prev_gmax;
-            radius /= decf; decf *= 2.0;
+        it.relative_decrease = tr.ev.quality(candidate_cost, mcc);
+        if (tr.successful(it.relative_decrease)) {
+          if (a.max_nonmonotonic > 0 && !(candidate_cost < min_cost) && best_is_current) {
+            for (int i = 0; i < kQParams; ++i) sx[2][i] = sx[0][i];    // leaving the best iterate: keep it
+            best_is_current = false;
+          } else if (a.max_nonmonotonic > 0 && candidate_cost < min_cost) {
+            best_is_current = true;
           }
+          for (int i = 0; i < kQParams; ++i) sx[0][i] = sx[1][i];
+          cur = 1 - cur;
+          x_cost = candidate_cost;
+          it.cost = x_cost;
+          it.gradient_max_norm = qba_gradmax(sg[cur], sx[0] + kMaxK, n);
+          it.step_is_successful = 1;
+          tr.accept(it.relative_decrease, candidate_cost, mcc);
+        } else {
+          it.step_is_successful = 0;
+          it.cost = candidate_cost;
+          it.gradient_max_norm = prev_gmax;
+          tr.reject();
         }
       }
       sctl[0] = act;
