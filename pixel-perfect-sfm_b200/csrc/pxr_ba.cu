@@ -340,8 +340,6 @@ int BA::create(pxr_ctx* c, const pxr_ba_desc* d, const pxr_interp_config* ic, co
   PXR_TRY(gc.alloc(nc));
   PXR_TRY(Hpp.alloc((size_t)n_points * 9)); PXR_TRY(gp.alloc((size_t)n_points * 3));
   h_obs_img.assign(d->obs_img, d->obs_img + n_obs);
-  // the monolithic kernel interpolates patches itself: a geometric handle always runs the batched rounds
-  use_monolithic_inner = std::getenv("PXR_INNER_MONOLITHIC") != nullptr && !geometric;
   if (for_solve) PXR_TRY(build_schur_pairs());
   if (block_mode) PXR_TRY(block_setup());
   if (for_solve && n_obs > 0 && n_obs < ((int64_t)1 << 31)) {
@@ -536,7 +534,6 @@ int BA::resident_setup(const pxr_ba_desc* d, size_t esz) {
   const int W = res_window;
   if (W < 4 || C < 8 || ph > 255 || pw > 255 || ph < W + 2 || pw < W + 2) return PXR_OK;       // nothing to gain / not representable
   if ((size_t)ph * pw * C * esz > staged_chunk_bytes()) return PXR_OK;      // a whole (shared) patch must fit a staging buffer
-  if (getenv("PXR_INNER_MONOLITHIC")) return PXR_OK;     // that kernel reads taps without the residency guard
   // the blocks must be HOST memory (a device-resident block needs no upload at all)
   auto is_device = [](const void* ptr) -> bool {
     cudaPointerAttributes pa;
@@ -1081,7 +1078,7 @@ int BA::eval_list(int set, const int64_t* list, int64_t n, const unsigned long l
   return PXR_OK;
 }
 
-// Inner iterations, batched: see pxr_inner.cuh.  Same state machine as ba_inner_kernel.
+// Inner iterations: see pxr_inner.cuh; the per-point rules are pxr_lm.cuh's.
 // Round 0's lists come from every variable point (round 0 itself evaluates every observation); from then on a round is
 // three launches (K0, K1, inner_step_kernel) and the step kernel builds the next round's lists.  Lists alternate between two buffers, counters rotate through three sets
 // (the step kernel of round r appends to set r+1 and zeroes set r+2, which no launch of round r touches).  The rounds are
@@ -1190,7 +1187,7 @@ int BA::capture_round_active() {
   return PXR_OK;
 }
 
-int BA::inner_iterations_batched(int set, double* trial_cost) {
+int BA::inner_iterations(int set, double* trial_cost) {
   if (n_points == 0 || n_obs == 0) return trial_cost ? fm_cost(trial_cost) : PXR_OK;
   StageScope stg(this, 9);
   cudaStream_t s = ctx->stream;
@@ -1216,26 +1213,6 @@ int BA::inner_iterations_batched(int set, double* trial_cost) {
     PXR_CUDA(cudaMemcpyAsync(X[set].p, inner_snapshot.p, (size_t)n_points * 24, cudaMemcpyDeviceToDevice, s));
   }
   return PXR_OK;
-}
-
-int BA::inner_iterations(int set, double* trial_cost) {
-  if (!use_monolithic_inner) return inner_iterations_batched(set, trial_cost);
-  if (trial_cost) {     // the monolithic kernel leaves no records behind: the cost takes a pass of its own
-    PXR_TRY(project(set, false, nullptr));
-    PXR_TRY(fm(0, nullptr, trial_cost));
-  }
-  InnerArgs a;
-  a.n_points = n_points; a.point_off = point_off.p; a.pt_begin = pt_begin.p;
-  a.obs_img = obs_img.p; a.obs_patch = obs_patch.p; a.img_cam = img_cam.p; a.cam_model = cam_model.p;
-  a.cam_params = cam[set].p; a.qvec = q[set].p; a.tvec = t[set].p; a.xyz = X[set].p;
-  a.corner = corner.p; a.scale = scale.p; a.ups = ups;
-  a.patches = d_patches; a.ph = ph; a.pw = pw;
-  a.refs = has_refs ? refs.p : nullptr;
-  a.loss.type = opt.loss_type; a.loss.a = opt.loss_scale;
-  a.l2_normalize = interp.l2_normalize;
-  if (n_points == 0) return PXR_OK;
-  StageScope st(this, 9);
-  return launch_inner(ctx, dtype, C, interp.use_float_simd != 0, a);
 }
 
 // ||set 0 - set 1||^2 (ambient), the step after inner iterations: points to scalars[11], cameras to scalars[12].  Only

@@ -28,7 +28,6 @@ namespace pxr {
 int fm_supported(int dtype, int C);
 int fm_max_partials(pxr_ctx* ctx);
 int launch_fm_eval(pxr_ctx* ctx, int dtype, int C, int mode, bool float_simd, const FmEvalArgs& a, int* n_partials);
-int launch_inner(pxr_ctx* ctx, int dtype, int C, bool float_simd, const InnerArgs& a);
 
 struct LMState {
   bool started = false, finished = false, pending_finalize = false, inner_enabled = false;
@@ -229,7 +228,6 @@ struct BA {
   int gradient_max_norm(double* out);
   // trial_cost (device scalar, optional): receives the cost at the starting point, reduced from round 0's records
   int inner_iterations(int set, double* trial_cost = nullptr);
-  int inner_iterations_batched(int set, double* trial_cost);
   int eval_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev = nullptr, bool settle = true,
                 cudaEvent_t after_k0 = nullptr, cudaEvent_t after_k1 = nullptr, int64_t k0_bound = -1);
   int alloc_inner_jpt();                            // inner_jpt's one allocation: before the rounds, or a debug entry
@@ -239,7 +237,7 @@ struct BA {
   int capture_round_lists(const int64_t* plist, const int64_t* list, const unsigned long long* cnt);
   int capture_round_active();
   int project_point_list(int set, const int64_t* list, int64_t n, const unsigned long long* n_dev, int64_t grid_bound);
-  int inner_rounds(int set, double* trial_cost);   // the <= 52 rounds of inner_iterations_batched, without a host wait per round
+  int inner_rounds(int set, double* trial_cost);   // the <= 52 rounds of inner_iterations, without a host wait per round
   unsigned long long* inner_cnt_host = nullptr;    // pinned, mapped [kInnerRounds][3]: each round's list lengths + the epoch of the call
   unsigned long long* inner_cnt_dev = nullptr;     // the same slots, device view (written by inner_step_kernel)
   unsigned long long inner_epoch = 0;              // incremented per inner_rounds call: tells this call's slots from stale ones
@@ -252,7 +250,6 @@ struct BA {
   DevBuf<int64_t> inner_list[2], inner_plist[2];   // a round's observation / point lists, alternating between rounds
   DevBuf<unsigned long long> inner_counters;       // 3 x [observations, points], rotating
   DevBuf<double> inner_jpt;                        // [n_obs][6]: d(uv)/dX of the observations a round evaluated
-  bool use_monolithic_inner = false;
   int step_norm_between_sets();                    // enqueues the squared point / camera parts to scalars[11] / [12]
   // LM driver (pxr_ba.cu), one loop for both modes; the three lm_* steps below are what differs with block_mode
   int lm_begin();

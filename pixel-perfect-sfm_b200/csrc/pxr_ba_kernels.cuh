@@ -9,6 +9,7 @@
 // (QuaternionManifold, SubsetManifold — bundle_optimizer.h:384-389,436-438).
 #pragma once
 #include "pxr_device.cuh"
+#include "pxr_lm.cuh"
 
 namespace pxr {
 
@@ -326,18 +327,17 @@ static __global__ void ba_diag_kernel(BADev d, double* diag) {
   }
 }
 
-// jacobi scaling (iteration 0): scale = 1/(1+sqrt(diag)) (ceres trust_region_minimizer.cc)
+// jacobi scaling (iteration 0)
 static __global__ void ba_scale_kernel(const double* diag, double* scale, int64_t n, int enabled) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) scale[i] = enabled ? 1.0 / (1.0 + sqrt(diag[i])) : 1.0;
+  if (i < n) scale[i] = enabled ? jacobi_scale(diag[i]) : 1.0;
 }
-// LM diagonal in unscaled variables: D2 = clamp(diag*scale^2, lo, hi) / (radius*scale^2)
+// LM diagonal in unscaled variables
 static __global__ void ba_d2_kernel(const double* diag, const double* scale, double* D2, int64_t n, double radius,
                              double lo, double hi) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double s2 = scale[i] * scale[i];
-  D2[i] = fmin(fmax(diag[i] * s2, lo), hi) / (radius * s2);
+  D2[i] = lm_damping(diag[i], scale[i], radius, lo, hi);
 }
 
 // S = Hcc + diag(D2c) (lower), rhs = -gc
@@ -353,29 +353,6 @@ static __global__ void ba_init_reduced_kernel(const double* Hcc, const double* g
     S[i] = v;
   }
   if (i < nc) rhs[i] = -gc[i];
-}
-
-__device__ __forceinline__ bool inv3_sym(const double* H, const double* D2, double inv[9]) {
-  const double a = H[0] + D2[0], b = H[1], c = H[2], dd = H[4] + D2[1], e = H[5], f = H[8] + D2[2];
-  if (!(a > 0.0)) return false;
-  const double l00 = sqrt(a), l10 = b / l00, l20 = c / l00;
-  const double t11 = dd - l10 * l10;
-  if (!(t11 > 0.0)) return false;
-  const double l11 = sqrt(t11), l21 = (e - l20 * l10) / l11;
-  const double t22 = f - l20 * l20 - l21 * l21;
-  if (!(t22 > 0.0)) return false;
-  const double l22 = sqrt(t22);
-  const double i00 = 1.0 / l00, i11 = 1.0 / l11, i22 = 1.0 / l22;
-  const double i10 = -l10 * i00 * i11;
-  const double i21 = -l21 * i11 * i22;
-  const double i20 = -(l20 * i00 + l21 * i10) * i22;
-  inv[0] = i00 * i00 + i10 * i10 + i20 * i20;
-  inv[1] = inv[3] = i10 * i11 + i20 * i21;
-  inv[2] = inv[6] = i20 * i22;
-  inv[4] = i11 * i11 + i21 * i21;
-  inv[5] = inv[7] = i21 * i22;
-  inv[8] = i22 * i22;
-  return true;
 }
 
 // K3: per-point Schur elimination without per-entry atomics.

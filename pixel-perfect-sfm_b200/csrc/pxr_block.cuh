@@ -59,9 +59,8 @@ static __global__ void __launch_bounds__(256) blk_post_kernel(GatherMap dg, cons
     double v = 0.0;
     for (int64_t j = dg.ptr[i]; j < dg.ptr[i + 1]; ++j) v += buf[dg.src[j]];
     diag[i] = v;
-    if (set_scale) jscale[i] = jacobi_scaling ? 1.0 / (1.0 + sqrt(v)) : 1.0;
-    const double s2 = jscale[i] * jscale[i];
-    D2[i] = fmin(fmax(v * s2, lo), hi) / (radius * s2);
+    if (set_scale) jscale[i] = jacobi_scaling ? jacobi_scale(v) : 1.0;
+    D2[i] = lm_damping(v, jscale[i], radius, lo, hi);
     rhs[i] = -gc[i] + rhsS[i];
     m = fabs(gc[i]);
   }

@@ -418,7 +418,7 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
     __syncthreads();
     return t;
   };
-  for (int i = tid; i < n; i += kKAThreads) w.scale[i] = a.jacobi_scaling ? 1.0 / (1.0 + sqrt(w.H[hdiag(i)])) : 1.0;
+  for (int i = tid; i < n; i += kKAThreads) w.scale[i] = a.jacobi_scaling ? jacobi_scale(w.H[hdiag(i)]) : 1.0;
   { double v = 0; for (int i = tid; i < n; i += kKAThreads) v += w.x[i] * w.x[i]; const double t = block_sum(v); if (tid == 0) w.ctrl[C_XNORM] = sqrt(t); }
   reduce_max_proj_grad();
   if (tid == 0) {
@@ -447,8 +447,7 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
     const double radius = w.ctrl[C_RADIUS];
     // ---- LM step: (H + D) delta = -g
     for (int i = tid; i < n; i += kKAThreads) {
-      const double s2 = w.scale[i] * w.scale[i];
-      w.D2[i] = fmin(fmax(w.H[hdiag(i)] * s2, a.min_diag), a.max_diag) / (radius * s2);
+      w.D2[i] = lm_damping(w.H[hdiag(i)], w.scale[i], radius, a.min_diag, a.max_diag);
       w.delta[i] = -w.g[i];
     }
     __syncthreads();

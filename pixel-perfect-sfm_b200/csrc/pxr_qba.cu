@@ -250,7 +250,7 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
   TrustRegion tr;
   double xn_points = 0.0;     // ||X||^2 of the constant points: part of ceres' ||x|| (ba_plus_kernel)
   if (tid == 0) {
-    for (int i = 0; i < n; ++i) sscale[i] = a.jacobi_scaling ? 1.0 / (1.0 + sqrt(sH[0][qtri(i, i)])) : 1.0;
+    for (int i = 0; i < n; ++i) sscale[i] = a.jacobi_scaling ? jacobi_scale(sH[0][qtri(i, i)]) : 1.0;
     for (int64_t o = ob; o < oe; ++o)
       for (int k = 0; k < 3; ++k) { const double x = a.xyz[3 * o + k]; xn_points += x * x; }
     it.cost = x_cost;
@@ -280,16 +280,13 @@ __global__ void __launch_bounds__(kQThreads) qba_solve_kernel(QBAArgs a) {
         it = pxr_iteration_summary();
         it.iteration = iteration;
         pending = true;
-        // ---- LM step: (H + D) delta = -g, D = clamp(diag(H) s^2, lo, hi) / (radius s^2)   (ba_d2_kernel)
+        // ---- LM step: (H + D) delta = -g, D = lm_damping of diag(H)
         const double* H = sH[cur];
         const double* g = sg[cur];
         double* L = sL;
         double* d = sd;
         for (int i = 0; i < n * (n + 1) / 2; ++i) L[i] = H[i];
-        for (int i = 0; i < n; ++i) {
-          const double s2 = sscale[i] * sscale[i];
-          L[qtri(i, i)] += fmin(fmax(H[qtri(i, i)] * s2, a.min_diag), a.max_diag) / (tr.radius * s2);
-        }
+        for (int i = 0; i < n; ++i) L[qtri(i, i)] += lm_damping(H[qtri(i, i)], sscale[i], tr.radius, a.min_diag, a.max_diag);
         bool ok = true;
         for (int j = 0; j < n && ok; ++j) {
           double djj = L[qtri(j, j)];

@@ -120,12 +120,7 @@ def test_full_solve_matches_oracle(inner):
     assert s_gpu["kernel_launches"] > 0
 
 
-@pytest.mark.parametrize("monolithic", [False, True])
-def test_inner_iterations_kernel_matches_oracle_points(monolithic, monkeypatch):
-    if monolithic:
-        monkeypatch.setenv("PXR_INNER_MONOLITHIC", "1")
-    else:
-        monkeypatch.delenv("PXR_INNER_MONOLITHIC", raising=False)
+def test_inner_iterations_kernel_matches_oracle_points():
     prob, gt, ic = _scene(n_points=30)
     prob.xyz += np.random.default_rng(5).normal(0, 0.004, prob.xyz.shape)
     so = _capi.default_ba_options(use_inner_iterations=1)

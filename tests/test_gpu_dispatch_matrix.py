@@ -34,7 +34,7 @@ def _cached(key, fn):
 
 def _set_env(monkeypatch, env):
     for k in ("PXR_SCHUR_KERNEL", "PXR_SCHUR_CTAS", "PXR_BUILD_ATOMIC", "PXR_BUILD_UNSTAGED", "PXR_PROJECT_UNSTAGED",
-              "PXR_PCG_SPARSE", "PXR_BLOCK_ASSEMBLY", "PXR_NO_SPECULATION", "PXR_INNER_MONOLITHIC"):
+              "PXR_PCG_SPARSE", "PXR_BLOCK_ASSEMBLY", "PXR_NO_SPECULATION"):
         monkeypatch.delenv(k, raising=False)
     for k, v in env.items():
         monkeypatch.setenv(k, v)
@@ -154,11 +154,10 @@ def test_block_sparse_assembly_matches_dense_and_oracle(name, env, monkeypatch):
     _compare_solutions(p_got, p_ref, 1e-4 if pcg else 1e-6)
 
 
-@pytest.mark.parametrize("inner_env", [{}, {"PXR_INNER_MONOLITHIC": "1"}], ids=["batched", "monolithic"])
 @pytest.mark.parametrize("name", ["dup_obs", "multi_chunk", "mixed_dc8"])
-def test_full_solve_with_inner_iterations_matches_oracle(name, inner_env, monkeypatch):
+def test_full_solve_with_inner_iterations_matches_oracle(name, monkeypatch):
     """the whole LM loop, inner iterations included, on the scenes whose pair structure is unusual"""
-    _set_env(monkeypatch, inner_env)
+    _set_env(monkeypatch, {})
     so = _capi.default_ba_options(use_inner_iterations=1, max_num_iterations=10)
     s_ref, p_ref = _cached(("oracle_full", name), lambda: _solve(name, O.ba_solve, so))
     s_gpu, p_gpu = _solve(name, _engine.ba_run, so)
@@ -179,12 +178,11 @@ def test_inner_iterations_on_duplicate_observations(monkeypatch):
     p_ref = prob.copy()
     O.lib().orc_ba_inner_iterations(C.byref(p_ref.desc()), C.byref(ic), C.byref(so))
     assert np.abs(p_ref.xyz - prob.xyz).max() > 1e-5
-    for env in ({}, {"PXR_INNER_MONOLITHIC": "1"}):
-        _set_env(monkeypatch, env)
-        h = _engine.BAHandle(prob.copy(), ic, so)
-        h.debug_inner_iterations()
-        h.read_params()
-        assert np.abs(h.problem.xyz - p_ref.xyz).max() < 1e-7, env
+    _set_env(monkeypatch, {})
+    h = _engine.BAHandle(prob.copy(), ic, so)
+    h.debug_inner_iterations()
+    h.read_params()
+    assert np.abs(h.problem.xyz - p_ref.xyz).max() < 1e-7
 
 
 def _rejecting_scene():

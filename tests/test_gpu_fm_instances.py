@@ -48,7 +48,7 @@ def _id(v):
 
 @pytest.mark.parametrize("ph,pw", PATCH_SHAPES, ids=lambda v: str(v))
 @pytest.mark.parametrize("dtype,channels", FM_INSTANCES, ids=_id)
-def test_fm_instance_matches_oracle(dtype, channels, ph, pw, monkeypatch):
+def test_fm_instance_matches_oracle(dtype, channels, ph, pw):
     prob = _ba_scene(dtype, channels, ph, pw)
     ic = _capi.default_interp()
     assert (prob.ph, prob.pw) == (ph, pw)
@@ -73,21 +73,16 @@ def test_fm_instance_matches_oracle(dtype, channels, ph, pw, monkeypatch):
         # clamped, and the per-point solve walks projections out of it (tens of pixels): where such an ill-posed solve
         # stops is not a property of the kernels.  The evaluation above covers these shapes.
         return
-    # one inner-iteration pass over the points, batched and monolithic
+    # one inner-iteration pass over the points
     prob.xyz += np.random.default_rng(5).normal(0, 0.004, prob.xyz.shape)
     so = _capi.default_ba_options(use_inner_iterations=1)
     p_ref = prob.copy()
     O.lib().orc_ba_inner_iterations(C.byref(p_ref.desc()), C.byref(ic), C.byref(so))
     assert np.abs(p_ref.xyz - prob.xyz).max() > 1e-5
-    for monolithic in (False, True):
-        if monolithic:
-            monkeypatch.setenv("PXR_INNER_MONOLITHIC", "1")
-        else:
-            monkeypatch.delenv("PXR_INNER_MONOLITHIC", raising=False)
-        h = _engine.BAHandle(prob.copy(), ic, so)
-        h.debug_inner_iterations()
-        h.read_params()
-        assert np.abs(h.problem.xyz - p_ref.xyz).max() < 1e-7, "monolithic" if monolithic else "batched"
+    h = _engine.BAHandle(prob.copy(), ic, so)
+    h.debug_inner_iterations()
+    h.read_params()
+    assert np.abs(h.problem.xyz - p_ref.xyz).max() < 1e-7
 
 
 def _ka(dtype, channels, ps):

@@ -141,17 +141,6 @@ def test_inner_iterations_match_oracle_points():
     assert np.abs(p_ref.xyz - prob.xyz).max() > 1e-5
 
 
-def test_monolithic_switch_has_no_effect(monkeypatch):
-    prob = _scene(n_points=50)
-    so = _capi.default_ba_options(use_inner_iterations=1, max_num_iterations=6)
-    p1, p2 = prob.copy(), prob.copy()
-    s1 = _engine.ba_run(p1, options=so)
-    monkeypatch.setenv("PXR_INNER_MONOLITHIC", "1")
-    s2 = _engine.ba_run(p2, options=so)
-    assert s1["num_inner_iteration_steps"] == s2["num_inner_iteration_steps"] > 0
-    assert np.abs(p1.xyz - p2.xyz).max() < 1e-9
-
-
 def test_eval_list_matches_full_range_records():
     prob = _scene(n_points=60)
     h = _engine.BAHandle(prob, options=_capi.default_ba_options())

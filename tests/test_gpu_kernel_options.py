@@ -44,7 +44,7 @@ def _ba_scene(dtype, channels, ph, pw):
     return F._ba_scene(dtype, channels, ph, pw)
 
 
-def _k1_and_inner(prob, ic, monkeypatch, monolithic_built=True):
+def _k1_and_inner(prob, ic):
     refs, _ = O.refs_compute(prob, ic)
     prob.refs = refs * 0.95 + 0.002
     so = _capi.default_ba_options(use_inner_iterations=0)
@@ -62,37 +62,27 @@ def _k1_and_inner(prob, ic, monkeypatch, monolithic_built=True):
     import ctypes as C
     O.lib().orc_ba_inner_iterations(C.byref(p_ref.desc()), C.byref(ic), C.byref(so))
     assert np.abs(p_ref.xyz - prob.xyz).max() > 1e-5
-    for monolithic in (False, True):
-        if monolithic:
-            monkeypatch.setenv("PXR_INNER_MONOLITHIC", "1")
-        else:
-            monkeypatch.delenv("PXR_INNER_MONOLITHIC", raising=False)
-        h = _engine.BAHandle(prob.copy(), ic, so)
-        if monolithic and not monolithic_built:
-            with pytest.raises((ValueError, _capi.PxrError), match="Unsupported dimensions"):
-                h.debug_inner_iterations()
-            continue
-        h.debug_inner_iterations()
-        h.read_params()
-        assert np.abs(h.problem.xyz - p_ref.xyz).max() < 1e-7, "monolithic" if monolithic else "batched"
+    h = _engine.BAHandle(prob.copy(), ic, so)
+    h.debug_inner_iterations()
+    h.read_params()
+    assert np.abs(h.problem.xyz - p_ref.xyz).max() < 1e-7
 
 
 @pytest.mark.parametrize("ph,pw", [(16, 16), (8, 8)], ids=str)
 @pytest.mark.parametrize("l2", [1, 0])
 @pytest.mark.parametrize("fs", [0, 1])
 @pytest.mark.parametrize("dtype,channels", FM_INSTANCES, ids=_id)
-def test_k1_and_inner_options(dtype, channels, fs, l2, ph, pw, monkeypatch):
+def test_k1_and_inner_options(dtype, channels, fs, l2, ph, pw):
     prob = _ba_scene(dtype, channels, ph, pw)
-    _k1_and_inner(prob, _capi.default_interp(l2_normalize=l2, use_float_simd=fs), monkeypatch)
+    _k1_and_inner(prob, _capi.default_interp(l2_normalize=l2, use_float_simd=fs))
 
 
 @pytest.mark.parametrize("dtype,channels", SMALL_INSTANCES, ids=_id)
-def test_k1_and_inner_small_channels_float_simd(dtype, channels, monkeypatch):
-    """the first C channels of a 16-channel scene: smooth, unnormalised maps as the cost maps are.  The monolithic
-    inner-iteration kernel is not built for these channel counts and refuses them."""
+def test_k1_and_inner_small_channels_float_simd(dtype, channels):
+    """the first C channels of a 16-channel scene: smooth, unnormalised maps as the cost maps are"""
     prob = _ba_scene(np.float64, 16, 16, 16)
     prob = prob.with_patches(np.ascontiguousarray(prob.patches[..., :channels].astype(dtype)))
-    _k1_and_inner(prob, _capi.default_interp(l2_normalize=0, use_float_simd=1), monkeypatch, monolithic_built=False)
+    _k1_and_inner(prob, _capi.default_interp(l2_normalize=0, use_float_simd=1))
 
 
 # ---- keypoint adjustment
