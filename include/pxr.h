@@ -505,7 +505,11 @@ int pxr_extract_patches(pxr_ctx* ctx, const void* dense, int32_t dense_on_device
 /* ---- featuremetric KA ---------------------------------------------------
  * replaces _keypoint_adjustment.FeatureMetricKeypointOptimizer.run
  * (keypoint_adjustment/bindings.cc:17-34; featuremetric_keypoint_optimizer.h:50-202;
- * keypoint_optimizer.h:110-157). Keypoints are IN/OUT. */
+ * keypoint_optimizer.h:110-157). Keypoints are IN/OUT.
+ * A problem may hold any number of keypoints; the normal equations are factored per connected component of its edges,
+ * and a component may hold at most 80 variable keypoints (else PXR_ERR_UNSUPPORTED, keypoints untouched).  A problem
+ * whose workspace does not fit in one block's shared memory is solved with its workspace in global memory; the
+ * summary message reports how many did. */
 typedef struct {
   int64_t n_keypoints;
   double* keypoints;            /* [n_keypoints][2] COLMAP image coords, in/out */

@@ -9,8 +9,9 @@
 //   loss      ceres::ScaledLoss(Cauchy, similarity) (featuremetric_keypoint_optimizer.h:191-196)
 //   bounds    KeypointOptimizerBase::ParameterizeKeypoints (keypoint_optimizer.h:110-157)
 //   solve     ceres::Solve: bounded Levenberg-Marquardt with projected Armijo line search
-//             (TrustRegionMinimizer::DoLineSearch), dense Cholesky in shared memory (the reference's
-//             SPARSE_NORMAL_CHOLESKY is an exact factorization too).
+//             (TrustRegionMinimizer::DoLineSearch), Cholesky per connected component of the problem (the
+//             reference's SPARSE_NORMAL_CHOLESKY is an exact factorization too); the workspace lives in shared
+//             memory, or in global memory for a problem whose workspace does not fit there.
 // Feature windows are re-read from L2 on every evaluation: after first touch a problem's working
 // set (<= 50 windows x 4 KiB) is cache resident, so KA is compute/L2 bound, not HBM bound.
 #include <algorithm>
@@ -53,11 +54,13 @@ struct KAArgs {
   // query mode (REF): every edge is (keypoint e_k1, fixed descriptor ref_desc[e_k2]); block-diagonal normal equations,
   // workspace in global memory so that a problem may hold any number of keypoints
   // dense mode: the normal equations are block diagonal over the connected components of the problem's edge graph
-  // (tracks packed into one problem do not couple); per variable the scalar range [lo, hi) of its component
-  const int32_t* var_blk_lo; const int32_t* var_blk_hi;   // [n_var]
+  // (tracks packed into one problem do not couple); per variable the scalar range [lo, hi) of its component and the
+  // offset of the component's packed lower triangle inside the problem's H and L
+  const int32_t* var_blk_lo; const int32_t* var_blk_hi; const int32_t* var_blk_off;   // [n_var]
   const double* ref_desc;           // [n_ref][C]
-  double* workspace; const int64_t* ws_off;   // per problem: 26 * nv doubles at workspace + ws_off[p]
-  int n_max;                        // max 2*nv over problems (shared memory sizing)
+  // per problem: its workspace (2 m + 10 n doubles, m = matrix size) at workspace + ws_off[p], or in shared memory
+  // where ws_off is NULL or ws_off[p] < 0
+  double* workspace; const int64_t* ws_off;
 };
 
 constexpr int kKAThreads = 256;
@@ -111,10 +114,12 @@ __device__ __forceinline__ GlobalWindow make_window(const KAArgs& a, int64_t kp,
   return w;
 }
 
-// Shared-memory workspace of one problem
+// Workspace of one problem: shared memory, or global memory for a problem too large for it
 struct KAWork {
-  double* H;      // packed lower, n(n+1)/2 : J^T J at x
-  double* L;      // packed lower           : factor of H + D
+  int m;          // doubles per matrix
+  const int32_t* blo; const int32_t* boff;   // the problem's var_blk_lo / var_blk_off
+  double* H;      // per component packed lower: J^T J at x (REF: h00, h10, h11 per keypoint)
+  double* L;      // per component packed lower: factor of H + D
   double* g;      // J^T r at x
   double* gq;     // gradient at a line-search trial point
   double* x; double* cand; double* delta; double* scale; double* D2; double* lo; double* hi; double* tmp;
@@ -133,13 +138,17 @@ __device__ double ka_evaluate(const KAArgs& a, const KAWork& w, int64_t eb, int6
   const bool active = lane < ACTIVE;
   __syncthreads();
   if (mode >= 1) for (int i = threadIdx.x; i < n; i += kKAThreads) gout[i] = 0.0;
-  if (mode == 2) for (int i = threadIdx.x; i < (REF ? 3 * (n / 2) : n * (n + 1) / 2); i += kKAThreads) w.H[i] = 0.0;
+  if (mode == 2) for (int i = threadIdx.x; i < w.m; i += kKAThreads) w.H[i] = 0.0;
   __syncthreads();
   double cost = 0.0;
   for (int64_t e = eb + warp; e < ee; e += kKAWarps) {
     const int64_t k1 = a.e_k1[e], k2 = a.e_k2[e];
     if (!REF && k1 == k2) continue;  // "Avoid optimizing a keypoint to itself" (topological_keypoint_optimizer.h:139-143)
     const int v1 = a.e_v1[e], v2 = REF ? -1 : a.e_v2[e];
+    // J^T J of the edge goes into its component's triangle (both variable endpoints lie in one component); the
+    // offsets are read here, where their latency hides behind the interpolation
+    int r0 = 0, hoff = 0;
+    if (!REF && mode == 2) { const int cv = v1 >= 0 ? v1 : v2; if (cv >= 0) { r0 = w.blo[cv]; hoff = w.boff[cv]; } }
     double p1[2], p2[2] = {0.0, 0.0};
     if (v1 >= 0) { p1[0] = xv[2 * v1]; p1[1] = xv[2 * v1 + 1]; } else { p1[0] = a.keypoints[2 * k1]; p1[1] = a.keypoints[2 * k1 + 1]; }
     if (!REF) { if (v2 >= 0) { p2[0] = xv[2 * v2]; p2[1] = xv[2 * v2 + 1]; } else { p2[0] = a.keypoints[2 * k2]; p2[1] = a.keypoints[2 * k2 + 1]; } }
@@ -214,11 +223,12 @@ __device__ double ka_evaluate(const KAArgs& a, const KAWork& w, int64_t eb, int6
               atomicAdd(&w.H[3 * v1 + 2], rho[1] * cf[1] * cf[1] * dd[1][1]);
             }
           } else {
+          double* Hc = w.H + hoff;
           for (int q = 0; q < 4; ++q)
             for (int t = 0; t < 4; ++t) {
               if (col[q] < 0 || col[t] < 0 || col[q] < col[t]) continue;
               if (col[q] == col[t] && q != t) continue;
-              atomicAdd(&w.H[tri(col[q], col[t])], rho[1] * cf[q] * cf[t] * dd[q][t]);
+              atomicAdd(&Hc[tri(col[q] - r0, col[t] - r0)], rho[1] * cf[q] * cf[t] * dd[q][t]);
             }
           }
         }
@@ -233,10 +243,11 @@ __device__ double ka_evaluate(const KAArgs& a, const KAWork& w, int64_t eb, int6
   return total;
 }
 
-// Block-diagonal variants: one warp per connected component [r0, r1) of the packed lower matrix.  The components of a
-// packed KA problem are its tracks (a handful of keypoints each), so this replaces an O(n^3) factorisation of the whole
-// problem (n up to 160) by many tiny ones that run in parallel.
-__device__ bool ka_cholesky_blocks(double* L, int n, const int32_t* bhi, double* ctrl_flag) {
+// Block-diagonal variants: one warp per connected component [r0, r1) of the matrix, whose packed lower triangle starts
+// at boff.  The components of a packed KA problem are its tracks (a handful of keypoints each), so this replaces an
+// O(n^3) factorisation of the whole problem by many tiny ones that run in parallel; a component holds at most 160
+// scalars.
+__device__ bool ka_cholesky_blocks(double* L, int n, const int32_t* bhi, const int32_t* boff, double* ctrl_flag) {
   if (threadIdx.x == 0) *ctrl_flag = 0.0;
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -244,18 +255,20 @@ __device__ bool ka_cholesky_blocks(double* L, int n, const int32_t* bhi, double*
     const int r1 = bhi[r0 >> 1];
     // every warp walks the same block list; the block starting at variable v belongs to warp v % kKAWarps
     if (((r0 >> 1) % kKAWarps) == warp) {
-      for (int j = r0; j < r1; ++j) {
-        double d = L[tri(j, j)];
+      double* Lc = L + boff[r0 >> 1];
+      const int nb = r1 - r0;
+      for (int j = 0; j < nb; ++j) {
+        double d = Lc[tri(j, j)];
         if (!(d > 0.0) || !isfinite(d)) { if (lane == 0) *ctrl_flag = 1.0; d = 1.0; }
         const double dj = sqrt(d);
         __syncwarp();
-        if (lane == 0) L[tri(j, j)] = dj;
-        for (int i = j + 1 + lane; i < r1; i += 32) L[tri(i, j)] /= dj;
+        if (lane == 0) Lc[tri(j, j)] = dj;
+        for (int i = j + 1 + lane; i < nb; i += 32) Lc[tri(i, j)] /= dj;
         __syncwarp();
-        const int m = r1 - (j + 1);
+        const int m = nb - (j + 1);
         for (int e = lane; e < m * m; e += 32) {
           const int i = j + 1 + e / m, k = j + 1 + e % m;
-          if (k <= i) L[tri(i, k)] -= L[tri(i, j)] * L[tri(k, j)];
+          if (k <= i) Lc[tri(i, k)] -= Lc[tri(i, j)] * Lc[tri(k, j)];
         }
         __syncwarp();
       }
@@ -265,24 +278,27 @@ __device__ bool ka_cholesky_blocks(double* L, int n, const int32_t* bhi, double*
   __syncthreads();
   return *ctrl_flag == 0.0;
 }
-__device__ void ka_chol_solve_blocks(const double* L, int n, const int32_t* bhi, double* b) {
+__device__ void ka_chol_solve_blocks(const double* L, int n, const int32_t* bhi, const int32_t* boff, double* b) {
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int r0 = 0; r0 < n;) {
     const int r1 = bhi[r0 >> 1];
     if (((r0 >> 1) % kKAWarps) == warp) {
-      for (int i = r0; i < r1; ++i) {
+      const double* Lc = L + boff[r0 >> 1];
+      double* bc = b + r0;
+      const int nb = r1 - r0;
+      for (int i = 0; i < nb; ++i) {
         double sacc = 0.0;
-        for (int k = r0 + lane; k < i; k += 32) sacc += L[tri(i, k)] * b[k];
+        for (int k = lane; k < i; k += 32) sacc += Lc[tri(i, k)] * bc[k];
         sacc = warp_sum(sacc);
-        if (lane == 0) b[i] = (b[i] - sacc) / L[tri(i, i)];
+        if (lane == 0) bc[i] = (bc[i] - sacc) / Lc[tri(i, i)];
         __syncwarp();
       }
-      for (int i = r1 - 1; i >= r0; --i) {
+      for (int i = nb - 1; i >= 0; --i) {
         double sacc = 0.0;
-        for (int k = i + 1 + lane; k < r1; k += 32) sacc += L[tri(k, i)] * b[k];
+        for (int k = i + 1 + lane; k < nb; k += 32) sacc += Lc[tri(k, i)] * bc[k];
         sacc = warp_sum(sacc);
-        if (lane == 0) b[i] = (b[i] - sacc) / L[tri(i, i)];
+        if (lane == 0) bc[i] = (bc[i] - sacc) / Lc[tri(i, i)];
         __syncwarp();
       }
     }
@@ -354,32 +370,40 @@ __device__ double ka_min_interp_poly(const KASample* smp, int ns, double xmin, d
 }
 
 enum { C_STOP = 0, C_RADIUS, C_DECF, C_XCOST, C_CURCOST, C_XNORM, C_GMAX, C_MCC, C_CAND, C_TMP, C_TMP2, C_FLAG, C_N };
+constexpr size_t kKACtrlBytes = (kKAWarps + C_N) * sizeof(double);   // wcost + ctrl: on chip in every launch
 
-template <typename T, int C, bool FS, bool REF>
+// GWS: the launch over the problems whose workspace is in global memory (ws_off[p] >= 0; query mode: all of them); the
+// other launch takes the rest, with its workspace in shared memory.  Two instances keep the on-chip one's accesses in
+// the shared state space.
+template <typename T, int C, bool FS, bool REF, bool GWS = REF>
 __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
   extern __shared__ __align__(16) double sm[];
-  auto hdiag = [](int i) { return REF ? 3 * (i >> 1) + ((i & 1) ? 2 : 0) : tri(i, i); };
   const int p = blockIdx.x;
   if (p >= a.n_problems) return;
+  const int64_t wo = a.ws_off ? a.ws_off[p] : -1;
+  if (GWS != (wo >= 0)) return;
   const int64_t eb = a.prob_edge_begin[p], ee = a.prob_edge_begin[p + 1];
   const int vb = a.prob_var_begin[p];
   const int nv = a.prob_var_begin[p + 1] - vb;
   const int n = 2 * nv;
-  const int nmax = a.n_max;
+  auto hdiag = [&](int i) {
+    if (REF) return 3 * (i >> 1) + ((i & 1) ? 2 : 0);
+    const int v = vb + (i >> 1), l = i - a.var_blk_lo[v];
+    return a.var_blk_off[v] + tri(l, l);
+  };
   KAWork w;
-  if (REF) {
-    double* q = a.workspace + a.ws_off[p];           // global memory: n is not bounded in query mode
-    w.H = q; q += 3 * nv; w.L = q; q += 3 * nv;
+  w.m = 3 * nv;                    // REF: (h00, h10, h11) per keypoint; dense: the components' triangles back to back
+  if (!REF && nv > 0) {
+    const int v = vb + nv - 1, nb = a.var_blk_hi[v] - a.var_blk_lo[v];
+    w.m = a.var_blk_off[v] + nb * (nb + 1) / 2;
+  }
+  w.blo = a.var_blk_lo + vb; w.boff = a.var_blk_off + vb;
+  w.wcost = sm; w.ctrl = sm + kKAWarps;
+  {
+    double* q = GWS ? a.workspace + wo : sm + kKAWarps + C_N;
+    w.H = q; q += w.m; w.L = q; q += w.m;
     w.g = q; q += n; w.gq = q; q += n; w.x = q; q += n; w.cand = q; q += n; w.delta = q; q += n;
     w.scale = q; q += n; w.D2 = q; q += n; w.lo = q; q += n; w.hi = q; q += n; w.tmp = q; q += n;
-    w.wcost = sm; w.ctrl = sm + kKAWarps;
-  } else {
-    double* q = sm;
-    const int tsz = nmax * (nmax + 1) / 2;
-    w.H = q; q += tsz; w.L = q; q += tsz;
-    w.g = q; q += nmax; w.gq = q; q += nmax; w.x = q; q += nmax; w.cand = q; q += nmax; w.delta = q; q += nmax;
-    w.scale = q; q += nmax; w.D2 = q; q += nmax; w.lo = q; q += nmax; w.hi = q; q += nmax; w.tmp = q; q += nmax;
-    w.wcost = q; q += kKAWarps; w.ctrl = q; q += C_N;
   }
   const int tid = threadIdx.x;
   double* out = a.prob_out + (int64_t)p * 6;
@@ -479,18 +503,21 @@ __global__ void __launch_bounds__(kKAThreads) ka_solve_kernel(KAArgs a) {
     } else {
     const int32_t* blo = a.var_blk_lo + vb;
     const int32_t* bhi = a.var_blk_hi + vb;
-    for (int i = tid; i < n * (n + 1) / 2; i += kKAThreads) w.L[i] = w.H[i];
+    const int32_t* boff = a.var_blk_off + vb;
+    for (int i = tid; i < w.m; i += kKAThreads) w.L[i] = w.H[i];
     __syncthreads();
-    for (int i = tid; i < n; i += kKAThreads) w.L[tri(i, i)] += w.D2[i];
+    for (int i = tid; i < n; i += kKAThreads) w.L[hdiag(i)] += w.D2[i];
     __syncthreads();
-    valid = ka_cholesky_blocks(w.L, n, bhi, &w.ctrl[C_FLAG]);
+    valid = ka_cholesky_blocks(w.L, n, bhi, boff, &w.ctrl[C_FLAG]);
     if (valid) {
-      ka_chol_solve_blocks(w.L, n, bhi, w.delta);
+      ka_chol_solve_blocks(w.L, n, bhi, boff, w.delta);
       // model cost change = -g.d - d^T H d / 2 (H is block diagonal over the components)
       double part = 0.0;
       for (int i = tid; i < n; i += kKAThreads) {
         double hd = 0.0;
-        for (int j = blo[i >> 1]; j < bhi[i >> 1]; ++j) hd += (i >= j ? w.H[tri(i, j)] : w.H[tri(j, i)]) * w.delta[j];
+        const int r0 = blo[i >> 1];
+        const double* Hc = w.H + boff[i >> 1];
+        for (int j = r0; j < bhi[i >> 1]; ++j) hd += (i >= j ? Hc[tri(i - r0, j - r0)] : Hc[tri(j - r0, i - r0)]) * w.delta[j];
         part += w.g[i] * w.delta[i] + 0.5 * w.delta[i] * hd;
         if (!isfinite(w.delta[i])) part = nan("");
       }
@@ -607,9 +634,11 @@ static int launch_ka(pxr_ctx* ctx, bool fs, bool ref, const KAArgs& a, size_t sm
   } else if (fs) {
     PXR_CUDA(cudaFuncSetAttribute(ka_solve_kernel<T, C, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     PXR_LAUNCH(ctx, (ka_solve_kernel<T, C, true, false>), a.n_problems, kKAThreads, smem, a);
+    if (a.ws_off) PXR_LAUNCH(ctx, (ka_solve_kernel<T, C, true, false, true>), a.n_problems, kKAThreads, kKACtrlBytes, a);
   } else {
     PXR_CUDA(cudaFuncSetAttribute(ka_solve_kernel<T, C, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     PXR_LAUNCH(ctx, (ka_solve_kernel<T, C, false, false>), a.n_problems, kKAThreads, smem, a);
+    if (a.ws_off) PXR_LAUNCH(ctx, (ka_solve_kernel<T, C, false, false, true>), a.n_problems, kKAThreads, kKACtrlBytes, a);
   }
   PXR_CUDA(cudaGetLastError());
   return PXR_OK;
@@ -654,9 +683,12 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
   std::vector<int64_t> var_kp;
   std::vector<double> vlo, vhi;
   const bool constrained = d->bound > 0.0 || d->patches_are_sparse;
-  int n_max = 0;
+  int max_comp = 0;                     // variable keypoints of the largest component (dense mode)
   std::vector<int64_t> owner(d->n_keypoints, -1);
-  std::vector<int32_t> vblo, vbhi;      // per variable: scalar range of its connected component (dense mode)
+  // per variable: scalar range of its connected component and the offset of the component's packed triangle in the
+  // problem's matrices (dense mode); per problem: doubles per matrix
+  std::vector<int32_t> vblo, vbhi, vboff;
+  std::vector<int64_t> pm(P, 0);
   for (int p = 0; p < P; ++p) {
     std::unordered_map<int64_t, int> idx;
     const size_t v0 = var_kp.size();
@@ -710,17 +742,35 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
       if (ev1[e] >= 0) ev1[e] = newidx[ev1[e]];
       if (ev2[e] >= 0) ev2[e] = newidx[ev2[e]];
     }
+    int64_t m = 0;
     for (int i = 0; i < nvp;) {
       int jn = i + 1;
       while (jn < nvp && find(order[jn]) == find(order[i])) ++jn;
-      for (int q = i; q < jn; ++q) { vblo.push_back(2 * i); vbhi.push_back(2 * jn); }
+      for (int q = i; q < jn; ++q) { vblo.push_back(2 * i); vbhi.push_back(2 * jn); vboff.push_back((int32_t)m); }
+      const int64_t nb = 2 * (jn - i);
+      m += nb * (nb + 1) / 2;
+      max_comp = std::max(max_comp, jn - i);
+      if (m > INT32_MAX) return fail(PXR_ERR_UNSUPPORTED, "a KA problem's normal equations exceed 2^31 entries");
       i = jn;
     }
-    n_max = std::max(n_max, 2 * nvp);
+    pm[p] = refmode ? 3 * (int64_t)nvp : m;
   }
   pvb[P] = (int32_t)var_kp.size();
-  if (!refmode && n_max > 160) return fail(PXR_ERR_UNSUPPORTED, "a KA problem has %d variable keypoints (> 80 supported per problem)", n_max / 2);
-  n_max = std::max(n_max, 2);
+  // one warp factors one component (ka_cholesky_blocks)
+  if (!refmode && max_comp > 80)
+    return fail(PXR_ERR_UNSUPPORTED, "a KA problem has a connected component of %d variable keypoints (> 80 supported per component)", max_comp);
+  // placement: a problem whose workspace fits the opt-in shared memory of one block runs on chip, any other one gets
+  // its workspace in global memory (query mode: every problem, its size is not bounded)
+  int smem_optin = 0;
+  PXR_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+  std::vector<int64_t> wso(P, -1);
+  int64_t ws_words = 0, smem_words = 0;
+  int n_offchip = 0;
+  for (int p = 0; p < P; ++p) {
+    const int64_t words = 2 * pm[p] + 10 * 2 * (int64_t)(pvb[p + 1] - pvb[p]);
+    if (!refmode && (kKAWarps + C_N + words) * (int64_t)sizeof(double) <= smem_optin) smem_words = std::max(smem_words, words);
+    else { wso[p] = ws_words; ws_words += words; ++n_offchip; }
+  }
   // ---- upload
   DevBuf<int64_t> d_peb, d_k1, d_k2, d_varkp, d_kppatch;
   DevBuf<int32_t> d_pvb, d_v1, d_v2, d_corner;
@@ -733,8 +783,9 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
   if (d->edge_weight) PXR_TRY(d_w.upload(d->edge_weight, d->n_edges, s));
   PXR_TRY(d_varkp.upload(var_kp.data(), var_kp.size(), s));
   PXR_TRY(d_lo.upload(vlo.data(), vlo.size(), s)); PXR_TRY(d_hi.upload(vhi.data(), vhi.size(), s));
-  DevBuf<int32_t> d_vblo, d_vbhi;
+  DevBuf<int32_t> d_vblo, d_vbhi, d_vboff;
   PXR_TRY(d_vblo.upload(vblo.data(), vblo.size(), s)); PXR_TRY(d_vbhi.upload(vbhi.data(), vbhi.size(), s));
+  PXR_TRY(d_vboff.upload(vboff.data(), vboff.size(), s));
   PXR_TRY(d_kp.upload(d->keypoints, (size_t)d->n_keypoints * 2, s));
   if (d->kp_patch) PXR_TRY(d_kppatch.upload(d->kp_patch, d->n_keypoints, s));
   const int64_t n_patches = d->kp_patch ? d->n_patches : std::max(d->n_patches, d->n_keypoints);
@@ -760,7 +811,8 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
   KAArgs a;
   a.n_problems = P; a.prob_edge_begin = d_peb.p; a.prob_var_begin = d_pvb.p;
   a.e_k1 = d_k1.p; a.e_k2 = d_k2.p; a.e_v1 = d_v1.p; a.e_v2 = d_v2.p; a.e_w = d->edge_weight ? d_w.p : nullptr;
-  a.var_kp = d_varkp.p; a.var_lower = d_lo.p; a.var_upper = d_hi.p; a.var_blk_lo = d_vblo.p; a.var_blk_hi = d_vbhi.p;
+  a.var_kp = d_varkp.p; a.var_lower = d_lo.p; a.var_upper = d_hi.p;
+  a.var_blk_lo = d_vblo.p; a.var_blk_hi = d_vbhi.p; a.var_blk_off = d_vboff.p;
   a.keypoints = d_kp.p; a.kp_patch = d->kp_patch ? d_kppatch.p : nullptr;
   a.patches = dp; a.ph = d->ph; a.pw = d->pw; a.corner = d_corner.p; a.scale = d_scale.p; a.ups = d->upsampling_factor;
   a.loss.type = so.loss_type; a.loss.a = so.loss_scale; a.l2_normalize = ic.l2_normalize; a.constrained = constrained ? 1 : 0;
@@ -768,24 +820,22 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
   a.ftol = so.function_tolerance; a.gtol = so.gradient_tolerance; a.ptol = so.parameter_tolerance;
   a.min_rel_dec = so.min_relative_decrease; a.radius0 = so.initial_trust_region_radius; a.max_radius = so.max_trust_region_radius;
   a.min_radius = so.min_trust_region_radius; a.min_diag = so.min_lm_diagonal; a.max_diag = so.max_lm_diagonal;
-  a.jacobi_scaling = so.jacobi_scaling; a.prob_out = d_out.p; a.n_max = n_max;
+  a.jacobi_scaling = so.jacobi_scaling; a.prob_out = d_out.p;
   a.max_nonmonotonic = so.use_nonmonotonic_steps ? std::max(0, so.max_consecutive_nonmonotonic_steps) : 0;
-  // query mode: block-diagonal workspace in global memory, 26 doubles per variable keypoint
   DevBuf<double> d_ref, d_ws;
   DevBuf<int64_t> d_wsoff;
   a.ref_desc = nullptr; a.workspace = nullptr; a.ws_off = nullptr;
   if (refmode) {
-    std::vector<int64_t> wso(P + 1, 0);
-    for (int p = 0; p < P; ++p) wso[p + 1] = wso[p] + 26 * (int64_t)(pvb[p + 1] - pvb[p]);
     PXR_TRY(d_ref.upload(d->ref_desc, (size_t)d->n_ref_desc * C, s));
-    PXR_TRY(d_wsoff.upload(wso.data(), wso.size(), s));
-    PXR_TRY(d_ws.alloc((size_t)std::max<int64_t>(wso[P], 1)));
-    PXR_CUDA(cudaStreamSynchronize(s));   // wso goes out of scope
-    a.ref_desc = d_ref.p; a.workspace = d_ws.p; a.ws_off = d_wsoff.p;
+    a.ref_desc = d_ref.p;
     h2d += (double)d->n_ref_desc * C * 8;
   }
-  const size_t smem = refmode ? (size_t)(kKAWarps + C_N) * sizeof(double)
-                              : ((size_t)n_max * (n_max + 1) + 10 * (size_t)n_max + kKAWarps + C_N) * sizeof(double);
+  if (n_offchip > 0) {      // wso lives until the synchronisation after the launch
+    PXR_TRY(d_wsoff.upload(wso.data(), wso.size(), s));
+    PXR_TRY(d_ws.alloc((size_t)std::max<int64_t>(ws_words, 1)));
+    a.workspace = d_ws.p; a.ws_off = d_wsoff.p;
+  }
+  const size_t smem = (size_t)(kKAWarps + C_N + smem_words) * sizeof(double);
   const bool fs = ic.use_float_simd != 0;
   int rc = PXR_ERR_UNSUPPORTED;
   cudaEvent_t tev0 = nullptr, tev1 = nullptr;
@@ -814,7 +864,9 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
     summary->solve_time_s = summary->total_time_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     float kms = 0.f;
     cudaEventElapsedTime(&kms, tev0, tev1);
-    std::snprintf(summary->message, sizeof(summary->message), "%d problems, max %d LM iterations, solve kernel %.3f ms", P, iters, kms);
+    std::snprintf(summary->message, sizeof(summary->message),
+                  "%d problems, max %d LM iterations, solve kernel %.3f ms, %d with an off-chip workspace", P, iters, kms,
+                  n_offchip);
   }
   cudaEventDestroy(tev0); cudaEventDestroy(tev1);
   return PXR_OK;

@@ -159,6 +159,7 @@ class FeatureMetricKeypointOptimizer:
         nres = max(1, s["num_residuals"])
         logger.info("KA Time: %.4gs, cost change: %.6g --> %.6g", s["total_time_s"], np.sqrt(s["initial_cost"] / nres),
                     np.sqrt(s["final_cost"] / nres))
+        logger.info("KA solve: %s", s["message"])   # problems, LM iterations, kernel time, problems solved off chip
         return True
 
     def summary(self):
