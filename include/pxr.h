@@ -326,6 +326,19 @@ int pxr_ba_evaluate_jacobians(pxr_ba* ba, double* residuals, double* grad, doubl
  * return the full step `delta` [n_local] and the model cost change.  Any output may be NULL. */
 int pxr_ba_debug_linearize(pxr_ba* ba, double radius, double* cost, double* Hcc, double* gc, double* Hpp,
                            double* gp, double* S, double* rhs, double* delta, double* model_cost_change);
+/* The reduced camera solve S x = rhs alone (tests), on a caller's system: S [nc][nc] row-major (only the lower triangle
+ * is read) and rhs [nc] are written where the LM step assembles them, then the handle's configured solver runs (dense
+ * Cholesky, its path chosen by PXR_CHOL_BAND / PXR_CHOL_MULTIKERNEL, or the dense PCG for ITERATIVE_SCHUR, PXR_CG_MULTI).
+ *  x       [nc]        the solution
+ *  factor  [nc+1][nc]  optional, Cholesky paths only: L in the lower triangle, row nc = L^-1 rhs (the upper triangle
+ *                      holds whatever S held there)
+ *  status              0 solved, 1 numerical failure (non-positive pivot, failed preconditioner), 2 the persistent
+ *                      Cholesky bailed out of a wait
+ *  linear_iterations   CG iterations (1 for the Cholesky), 0 when the preconditioner failed.
+ * The block-sparse and block-mode paths have no dense S: PXR_ERR_UNSUPPORTED.  factor, status and linear_iterations
+ * may be NULL. */
+int pxr_ba_debug_reduced_solve(pxr_ba* ba, const double* S, const double* rhs, double* x, double* factor, int* status,
+                               int* linear_iterations);
 /* Runs the per-point inner iterations (ceres CoordinateDescentMinimizer equivalent) once on the
  * current parameters (parity tests). */
 int pxr_ba_debug_inner_iterations(pxr_ba* ba);

@@ -249,6 +249,21 @@ int orc_ba_layout(const pxr_ba_desc* d, int* n_cam_local, int* n_local, int* pos
   return 0;
 }
 
+// SchurJacobiPCG on a caller's system: S [n][n] symmetric, full storage; the preconditioner blocks are
+// [blk_off[k], blk_off[k] + blk_dim[k]).  x [n], iterations and stop_reason (PCGStop: 0 zeta test, 1 p.q <= 0,
+// 2 iteration cap, 3 failure).  Returns 0 when the solve succeeded, 1 on failure (as the oracle's step reports it).
+int orc_schur_jacobi_pcg(int n, const double* S, const double* b, int n_blocks, const int32_t* blk_off,
+                         const int32_t* blk_dim, int max_iter, double eta, double* x, int* iterations, int* stop_reason) {
+  std::vector<double> Sv(S, S + (size_t)n * n), bv(b, b + n), xv;
+  std::vector<std::pair<int, int>> blocks;
+  for (int k = 0; k < n_blocks; ++k) blocks.emplace_back(blk_off[k], blk_dim[k]);
+  int it = 0, stop = kPCGFailure;
+  const bool ok = SchurJacobiPCG(n, Sv, bv, blocks, max_iter, eta, &xv, &it, &stop);
+  for (int i = 0; i < n; ++i) x[i] = (size_t)i < xv.size() ? xv[i] : 0.0;   // a failed block inverse leaves xv empty
+  *iterations = it; *stop_reason = stop;
+  return ok ? 0 : 1;
+}
+
 // Linearise at the current parameters with the full (un-shortcut) Jacobians and run ONE
 // LM step computation at the given radius (jacobi scaling taken from this linearisation, as
 // in iteration 0).  Outputs (any may be NULL): Hcc [nc*nc], gc [nc], Hpp [np*9], gp [np*3],

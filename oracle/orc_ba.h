@@ -253,10 +253,15 @@ struct BAEvalOptions {
 
 // (ceres) ConjugateGradientsSolver::Solve (internal/ceres/conjugate_gradients_solver.cc @2.1) on the explicit
 // damped Schur complement S (symmetric, full storage) with the SCHUR_JACOBI preconditioner = inverse of the
-// diagonal blocks of S (one block per camera-side parameter block).  x starts at 0.
+// diagonal blocks of S (one block per camera-side parameter block).  x starts at 0.  stop_out (optional) tells why it
+// ended: PCGStop below.
+enum PCGStop { kPCGZeta = 0, kPCGNonPositiveCurvature = 1, kPCGMaxIterations = 2, kPCGFailure = 3 };
 inline bool SchurJacobiPCG(int n, const std::vector<double>& S, const std::vector<double>& b,
                            const std::vector<std::pair<int, int>>& blocks, int max_iter, double q_tolerance,
-                           std::vector<double>* xout, int* iters_out) {
+                           std::vector<double>* xout, int* iters_out, int* stop_out = nullptr) {
+  int stop_dummy = 0;
+  int& stop = stop_out ? *stop_out : stop_dummy;
+  stop = kPCGFailure;
   std::vector<double> Minv((size_t)n * 12, 0.0);  // row-wise storage of the block inverses (block dim <= 12)
   for (auto& bk : blocks) {
     const int o = bk.first, d = bk.second;
@@ -289,7 +294,7 @@ inline bool SchurJacobiPCG(int n, const std::vector<double>& S, const std::vecto
   x.assign(n, 0.0);
   *iters_out = 0;
   const double norm_b = std::sqrt(dot(b, b));
-  if (norm_b == 0.0) return true;
+  if (norm_b == 0.0) { stop = kPCGZeta; return true; }
   std::vector<double> r(b), z(n), p(n), q(n), tmp(n);
   double rho = 1.0, Q0 = 0.0;  // -0.5 * x.(b + r) with x = 0
   for (int it = 1;; ++it) {
@@ -301,7 +306,7 @@ inline bool SchurJacobiPCG(int n, const std::vector<double>& S, const std::vecto
     else { const double beta = rho / last_rho; if (beta == 0.0 || !std::isfinite(beta)) return false; for (int i = 0; i < n; ++i) p[i] = z[i] + beta * p[i]; }
     mul(p, q);
     const double pq = dot(p, q);
-    if (pq <= 0.0 || !std::isfinite(pq)) { *iters_out = it; break; }
+    if (pq <= 0.0 || !std::isfinite(pq)) { *iters_out = it; stop = kPCGNonPositiveCurvature; break; }
     const double alpha = rho / pq;
     if (!std::isfinite(alpha)) return false;
     for (int i = 0; i < n; ++i) x[i] += alpha * p[i];
@@ -311,9 +316,9 @@ inline bool SchurJacobiPCG(int n, const std::vector<double>& S, const std::vecto
     const double Q1 = -0.5 * xbr;
     const double zeta = it * (Q1 - Q0) / Q1;
     *iters_out = it;
-    if (zeta < q_tolerance) break;
+    if (zeta < q_tolerance) { stop = kPCGZeta; break; }
     Q0 = Q1;
-    if (it >= max_iter) break;
+    if (it >= max_iter) { stop = kPCGMaxIterations; break; }
   }
   return true;
 }

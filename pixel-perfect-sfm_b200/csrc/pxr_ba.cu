@@ -908,6 +908,17 @@ int BA::launch_sp_schur_pairs(const BADev& d, double* Bk, double* rhs_out, doubl
   return PXR_OK;
 }
 
+// Stage 5: S delta_c = rhs with the reduced system where the assembly leaves it (S / rhs, or the image blocks of the
+// block-sparse path), by the handle's solver: PCG or the dense Cholesky -> delta[0..nc).  A failure sets flags[1].
+int BA::solve_reduced() {
+  StageScope st(this, 5);
+  last_linear_iterations = 1;
+  if (nc == 0) return PXR_OK;
+  if (sparse_schur) return pcg_solve_sparse();
+  if (use_pcg) return pcg_solve();
+  return chol_launch();
+}
+
 // One LM step attempt at the current linearisation: fills delta, returns validity and model cost change
 int BA::compute_step(double radius, bool* valid, double* model_cost_change) {
   cudaStream_t s = ctx->stream;
@@ -943,16 +954,9 @@ int BA::compute_step(double radius, bool* valid, double* model_cost_change) {
     PXR_CUDA(cudaMemcpyAsync(rhs.p, S.p + (size_t)nc * nc, (size_t)nc * 8, cudaMemcpyDeviceToDevice, s));   // PCG / debug read rhs
   }
   }
-  st.reset(); st.reset(new StageScope(this, 5));
-  last_linear_iterations = 1;
-  if (nc > 0 && sparse_schur) {
-    PXR_TRY(pcg_solve_sparse());
-  } else if (nc > 0 && use_pcg) {
-    PXR_TRY(pcg_solve());
-  } else if (nc > 0) {
-    PXR_TRY(chol_launch());
-  }
-  st.reset(); st.reset(new StageScope(this, 7));
+  st.reset();
+  PXR_TRY(solve_reduced());
+  st.reset(new StageScope(this, 7));
   PXR_CUDA(cudaMemsetAsync(scalars.p + 4, 0, 4 * 8, s));  // acc[0..3]
   if (n_points > 0) PXR_LAUNCH(ctx, ba_backsub_kernel, (unsigned)cdiv(n_points * 32, 256), 256, 0, d, D2.p, delta.p);
   if (n_obs > 0) {
@@ -1245,8 +1249,13 @@ int BA::pcg_setup_blocks() {
   std::vector<int32_t> sd(off.size());
   for (size_t k = 0; k < off.size(); ++k) sd[k] = (k + 1 < off.size() ? off[k + 1] : nc) - off[k];
   cg_nblk = (int)off.size();
+  // every row's block (offset, dimension) depends on the layout only: the preconditioner kernels read it from here
+  std::vector<int32_t> row_off(nc), row_dim(nc);
+  for (size_t k = 0; k < off.size(); ++k)
+    for (int i = 0; i < sd[k]; ++i) { row_off[off[k] + i] = off[k]; row_dim[off[k] + i] = sd[k]; }
   PXR_TRY(cg_blk_off.upload(off.data(), off.size(), s)); PXR_TRY(cg_blk_dim.upload(sd.data(), sd.size(), s));
-  PXR_TRY(cg_Minv.alloc((size_t)nc * 12)); PXR_TRY(cg_row_off.alloc(nc)); PXR_TRY(cg_row_dim.alloc(nc));
+  PXR_TRY(cg_row_off.upload(row_off.data(), row_off.size(), s)); PXR_TRY(cg_row_dim.upload(row_dim.data(), row_dim.size(), s));
+  PXR_TRY(cg_Minv.alloc((size_t)nc * 12));
   PXR_TRY(cg_z.alloc(nc)); PXR_TRY(cg_p.alloc(nc)); PXR_TRY(cg_q.alloc(nc)); PXR_TRY(cg_r.alloc(nc)); PXR_TRY(cg_x.alloc(nc)); PXR_TRY(cg_tmp.alloc(nc));
   PXR_TRY(cg_state.alloc(1));
   if (sparse_schur) {
@@ -1286,7 +1295,7 @@ int BA::pcg_solve_sparse() {
   PXR_LAUNCH(ctx, sp_blockdiag_kernel, (unsigned)cdiv(((int64_t)n_images + ss_n_keys) * 8, 256), 256, 0, sp, ss_Dblk.p);
   if (ctx->world > 1) PXR_TRY(allreduce_f64(ctx, ss_Dblk.p, (size_t)cg_nblk * 144));
   PXR_LAUNCH(ctx, sp_block_inverse_kernel, (unsigned)cdiv(cg_nblk, 64), 64, 0, ss_Dblk.p, D2.p, 1, cg_blk_off.p, cg_blk_dim.p, cg_nblk,
-             cg_Minv.p, cg_row_off.p, cg_row_dim.p, flags.p + 1);
+             cg_Minv.p, flags.p + 1);
   return run_cg(spmv);
 }
 
@@ -1297,7 +1306,7 @@ int BA::pcg_solve() {
   const unsigned gv = (unsigned)cdiv((int64_t)n * 32, 256);
   PXR_LAUNCH(ctx, cg_mirror_kernel, (unsigned)cdiv((int64_t)n * n, 256), 256, 0, S.p, n);
   PXR_LAUNCH(ctx, cg_block_inverse_kernel, (unsigned)cdiv(cg_nblk, 64), 64, 0, S.p, n, cg_blk_off.p, cg_blk_dim.p, cg_nblk, cg_Minv.p,
-             cg_row_off.p, cg_row_dim.p, flags.p + 1);
+             flags.p + 1);
   auto spmv = [&](const double* x, double* y) -> int {
     PXR_LAUNCH(ctx, cg_gemv_kernel, gv, 256, 0, S.p, x, y, n, cg_state.p);
     return PXR_OK;
@@ -1307,7 +1316,8 @@ int BA::pcg_solve() {
 
 // Preconditioned CG on the reduced system given its product; Ceres' ConjugateGradientsSolver recurrences and
 // termination (Q-decrease ratio, residual refresh every 10 iterations).  Small systems run the single-CTA vector
-// kernels (deterministic sums); from 4096 unknowns the multi-CTA variants.
+// kernels (deterministic sums); from 4096 unknowns the multi-CTA variants.  The block inverse that ran before reports a
+// failure in flags[1]; the init kernels then finish the solve with 0 iterations.
 int BA::run_cg(const std::function<int(const double*, double*)>& spmv) {
   cudaStream_t s = ctx->stream;
   const int n = nc;
@@ -1316,11 +1326,11 @@ int BA::run_cg(const std::function<int(const double*, double*)>& spmv) {
   CGState hs;
   if (multi) {
     if (cg_part.n < (size_t)3 * gn) PXR_TRY(cg_part.alloc((size_t)3 * gn));
-    PXR_LAUNCH(ctx, cgm_init_state_kernel, 1, 1, 0, cg_state.p, opt.max_linear_solver_iterations, 0.1);
+    PXR_LAUNCH(ctx, cgm_init_state_kernel, 1, 1, 0, cg_state.p, opt.max_linear_solver_iterations, 0.1, flags.p + 1);
     PXR_LAUNCH(ctx, cgm_init_kernel, gn, 256, 0, rhs.p, cg_x.p, cg_r.p, n, cg_state.p, cg_part.p);
     PXR_LAUNCH(ctx, cgm_init_done_kernel, 1, 32, 0, cg_state.p, cg_part.p, (int)gn);
   } else {
-    PXR_LAUNCH(ctx, cg_init_kernel, 1, 1024, 0, rhs.p, cg_x.p, cg_r.p, n, cg_state.p, opt.max_linear_solver_iterations, 0.1);
+    PXR_LAUNCH(ctx, cg_init_kernel, 1, 1024, 0, rhs.p, cg_x.p, cg_r.p, n, cg_state.p, opt.max_linear_solver_iterations, 0.1, flags.p + 1);
   }
   for (int it = 0; it < opt.max_linear_solver_iterations; ++it) {
     const bool refresh = (it + 1) % 10 == 0;   // residual_reset_period
@@ -1971,6 +1981,41 @@ int pxr_ba_debug_linearize(pxr_ba* ba, double radius, double* cost, double* Hcc,
   if (delta) PXR_CUDA(cudaMemcpyAsync(delta, b->delta.p, (size_t)b->nl * 8, cudaMemcpyDeviceToHost, s));
   PXR_CUDA(cudaStreamSynchronize(s));
   if (model_cost_change) *model_cost_change = mcc;
+  return PXR_OK;
+}
+
+// The reduced solve on a caller's system (tests): S [nc][nc] (lower triangle read) and rhs go where compute_step's
+// assembly puts them, then BA::solve_reduced runs the handle's solver.
+int pxr_ba_debug_reduced_solve(pxr_ba* ba, const double* S, const double* rhs, double* x, double* factor, int* status,
+                               int* linear_iterations) {
+  if (!ba || !S || !rhs || !x) return fail(PXR_ERR_INVALID_ARGUMENT, "ba, S, rhs and x must not be NULL");
+  BA* b = reinterpret_cast<BA*>(ba);
+  if (b->sparse_schur || b->block_mode) return fail(PXR_ERR_UNSUPPORTED, "the block-sparse path has no dense S to solve");
+  pxr_ctx* ctx = b->ctx;
+  cudaStream_t s = ctx->stream;
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  const size_t nc = (size_t)b->nc;
+  if (nc > 0) {
+    PXR_CUDA(cudaMemcpyAsync(b->S.p, S, nc * nc * 8, cudaMemcpyHostToDevice, s));
+    PXR_CUDA(cudaMemcpyAsync(b->S.p + nc * nc, rhs, nc * 8, cudaMemcpyHostToDevice, s));   // row nc: the Cholesky's rhs
+    PXR_CUDA(cudaMemcpyAsync(b->rhs.p, rhs, nc * 8, cudaMemcpyHostToDevice, s));           // the PCG's
+  }
+  PXR_CUDA(cudaMemsetAsync(b->flags.p, 0, 4 * sizeof(int), s));
+  PXR_TRY(b->solve_reduced());
+  int fl[4] = {0, 0, 0, 0};
+  PXR_CUDA(cudaMemcpyAsync(fl, b->flags.p, sizeof(fl), cudaMemcpyDeviceToHost, s));
+  if (nc > 0) PXR_CUDA(cudaMemcpyAsync(x, b->delta.p, nc * 8, cudaMemcpyDeviceToHost, s));
+  if (factor && nc > 0 && !b->use_pcg) PXR_CUDA(cudaMemcpyAsync(factor, b->S.p, (nc + 1) * nc * 8, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
+  int st = fl[1] != 0 ? 1 : 0;
+  if (st && !b->use_pcg && b->chol_graph_exec && !b->chol_multikernel) {
+    // the persistent kernel raises the same flag when it bails out of a wait; its abort word tells the two apart
+    int aborted = 0;
+    PXR_CUDA(cudaMemcpy(&aborted, b->chol_sync.p + (pxr_chol::sync_ints((int)cdiv((int64_t)nc, kNB)) - 1), sizeof(int), cudaMemcpyDeviceToHost));
+    if (aborted) st = 2;
+  }
+  if (status) *status = st;
+  if (linear_iterations) *linear_iterations = b->last_linear_iterations;
   return PXR_OK;
 }
 

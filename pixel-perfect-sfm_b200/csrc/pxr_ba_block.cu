@@ -466,7 +466,7 @@ int BA::pcg_solve_block() {
   GatherMap gd{gmD_dest.p, gmD_ptr.p, gmD_src.p, gmD_rows};
   if (gmD_rows > 0) PXR_LAUNCH(ctx, blk_gather_kernel, (unsigned)cdiv(gmD_rows, 256), 256, 0, gd, G, ss_Dblk.p, (const double*)nullptr, 1);
   PXR_LAUNCH(ctx, sp_block_inverse_kernel, (unsigned)cdiv(cg_nblk, 64), 64, 0, ss_Dblk.p, D2.p, 1, cg_blk_off.p, cg_blk_dim.p, cg_nblk,
-             cg_Minv.p, cg_row_off.p, cg_row_dim.p, flags.p + 1);
+             cg_Minv.p, flags.p + 1);
   BlockRows br;
   br.chunk_begin = br_chunk_begin.p; br.chunk_img = br_chunk_img.p; br.chunk_first = br_chunk_first.p; br.ent_key = br_ent_key.p;
   br.n_chunks = br_n_chunks; br.cols = GatherMap{nullptr, br_cols_ptr.p, br_cols_src.p, nc};

@@ -115,6 +115,7 @@ struct BA {
   DevBuf<CGState> cg_state;
   int cg_nblk = 0, last_linear_iterations = 1;
   int pcg_solve();
+  int solve_reduced();               // stage 5 of compute_step: S delta_c = rhs by PCG or the dense Cholesky
   int run_cg(const std::function<int(const double*, double*)>& spmv);
   // implicit block-sparse reduced system (pxr_sparse_schur.cuh): no nc x nc array is ever allocated
   // debugging / A-B switches, read from the environment once in create()

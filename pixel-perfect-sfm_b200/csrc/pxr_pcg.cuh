@@ -23,9 +23,10 @@ static __global__ void cg_mirror_kernel(double* S, int n) {
   if (c > r) S[i] = S[(int64_t)c * n + r];
 }
 
-// inverse of every diagonal block (dim <= 12), one thread per block; Minv row-wise [n][12]
+// inverse of every diagonal block (dim <= 12), one thread per block; Minv row-wise [n][12].  A non-positive pivot sets
+// *fail and leaves the block's rows unwritten: the CG init kernels then end the solve before its first iteration.
 static __global__ void cg_block_inverse_kernel(const double* S, int n, const int32_t* blk_off, const int32_t* blk_dim, int nblk,
-                                               double* Minv, int32_t* row_off, int32_t* row_dim, int* fail) {
+                                               double* Minv, int* fail) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= nblk) return;
   const int o = blk_off[b], d = blk_dim[b];
@@ -41,10 +42,8 @@ static __global__ void cg_block_inverse_kernel(const double* S, int n, const int
       for (int j = 0; j < 2 * d; ++j) A[i][j] -= f * A[k][j];
     }
   }
-  for (int i = 0; i < d; ++i) {
-    row_off[o + i] = o; row_dim[o + i] = d;
+  for (int i = 0; i < d; ++i)
     for (int j = 0; j < d; ++j) Minv[(int64_t)(o + i) * 12 + j] = A[i][d + j];
-  }
 }
 
 // out = S v (S full, row-major), one warp per row
@@ -72,14 +71,17 @@ __device__ __forceinline__ double cta_sum(double v) {
   return t;
 }
 
-// init: x = 0, r = b, state
-static __global__ void __launch_bounds__(1024) cg_init_kernel(const double* b, double* x, double* r, int n, CGState* st, int max_iter, double q_tol) {
+// init: x = 0, r = b, state.  A failed preconditioner (*precond_fail, set by the block inverse) ends the solve here with
+// 0 iterations, as ceres' ConjugateGradientsSolver stops when the preconditioner update fails.
+static __global__ void __launch_bounds__(1024) cg_init_kernel(const double* b, double* x, double* r, int n, CGState* st, int max_iter, double q_tol,
+                                                              const int* precond_fail) {
   double nb = 0.0;
   for (int i = threadIdx.x; i < n; i += blockDim.x) { x[i] = 0.0; r[i] = b[i]; nb += b[i] * b[i]; }
   nb = cta_sum(nb);
   if (threadIdx.x == 0) {
-    st->rho = 1.0; st->last_rho = 1.0; st->alpha = 0; st->beta = 0; st->Q0 = 0.0; st->it = 0; st->failed = 0;
-    st->done = nb == 0.0 ? 1 : 0; st->max_iter = max_iter; st->q_tol = q_tol;
+    const int failed = *precond_fail != 0;
+    st->rho = 1.0; st->last_rho = 1.0; st->alpha = 0; st->beta = 0; st->Q0 = 0.0; st->it = 0; st->failed = failed;
+    st->done = (failed || nb == 0.0) ? 1 : 0; st->max_iter = max_iter; st->q_tol = q_tol;
   }
 }
 
@@ -172,8 +174,9 @@ static __global__ void __launch_bounds__(256) cgm_init_kernel(const double* b, d
   nb = cta_sum(nb);
   if (threadIdx.x == 0) part[2 * gridDim.x + blockIdx.x] = nb;
 }
-static __global__ void cgm_init_state_kernel(CGState* st, int max_iter, double q_tol) {   // before cgm_init_kernel
-  st->rho = 1.0; st->last_rho = 1.0; st->alpha = 0; st->beta = 0; st->Q0 = 0.0; st->it = 0; st->failed = 0; st->done = 0;
+static __global__ void cgm_init_state_kernel(CGState* st, int max_iter, double q_tol, const int* precond_fail) {   // before cgm_init_kernel
+  const int failed = *precond_fail != 0;         // failed preconditioner: done before the first iteration, as cg_init_kernel
+  st->rho = 1.0; st->last_rho = 1.0; st->alpha = 0; st->beta = 0; st->Q0 = 0.0; st->it = 0; st->failed = failed; st->done = failed;
   st->max_iter = max_iter; st->q_tol = q_tol; st->pq = 0.0; st->rz = 0.0; st->xbr = 0.0;
 }
 static __global__ void __launch_bounds__(32) cgm_init_done_kernel(CGState* st, const double* part, int g) {   // b == 0

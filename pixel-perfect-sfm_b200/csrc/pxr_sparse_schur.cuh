@@ -190,8 +190,7 @@ static __global__ void __launch_bounds__(256) sp_blockdiag_kernel(SparseSchur s,
 
 // invert the (damped) diagonal blocks: Dblk + diag(D2) -> Minv rows; same output layout as cg_block_inverse_kernel
 static __global__ void sp_block_inverse_kernel(const double* Dblk, const double* D2, int add_d2, const int32_t* blk_off,
-                                               const int32_t* blk_dim, int nblk, double* Minv, int32_t* row_off,
-                                               int32_t* row_dim, int* fail) {
+                                               const int32_t* blk_dim, int nblk, double* Minv, int* fail) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= nblk) return;
   const int o = blk_off[b], d = blk_dim[b];
@@ -211,10 +210,8 @@ static __global__ void sp_block_inverse_kernel(const double* Dblk, const double*
       for (int j = 0; j < 2 * d; ++j) A[i][j] -= f * A[k][j];
     }
   }
-  for (int i = 0; i < d; ++i) {
-    row_off[o + i] = o; row_dim[o + i] = d;
+  for (int i = 0; i < d; ++i)
     for (int j = 0; j < d; ++j) Minv[(int64_t)(o + i) * 12 + j] = A[i][d + j];
-  }
 }
 
 // rhs = -gc (the Schur part is added by ba_schur_prep_kernel)

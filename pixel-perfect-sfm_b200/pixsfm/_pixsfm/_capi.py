@@ -15,6 +15,8 @@ PXR_MAX_CAM_PARAMS = 12
 # util/src/log_exceptions.h:52-84; unsupported (C,N) -> std::invalid_argument)
 PXR_OK, PXR_ERR_INVALID_ARGUMENT, PXR_ERR_UNSUPPORTED, PXR_ERR_NO_DEVICE, PXR_ERR_CUDA, \
     PXR_ERR_NCCL, PXR_ERR_NUMERIC, PXR_ERR_INTERRUPTED, PXR_ERR_INTERNAL = range(9)
+# status of pxr_ba_debug_reduced_solve
+REDUCED_SOLVE_OK, REDUCED_SOLVE_FAILED, REDUCED_SOLVE_BAILED_OUT = range(3)
 
 CAMERA_MODEL_IDS = {"SIMPLE_PINHOLE": 0, "PINHOLE": 1, "SIMPLE_RADIAL": 2, "RADIAL": 3,
                     "OPENCV": 4, "OPENCV_FISHEYE": 5, "FULL_OPENCV": 6}

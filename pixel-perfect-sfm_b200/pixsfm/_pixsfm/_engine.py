@@ -76,6 +76,22 @@ class BAHandle:
         out["cost"] = cost.value; out["model_cost_change"] = mcc.value
         return out
 
+    def debug_reduced_solve(self, S, rhs, factor=False):
+        """pxr_ba_debug_reduced_solve: the handle's reduced-system solver on S x = rhs (S [nc, nc], lower triangle read)
+        -> dict(x, status (_capi.REDUCED_SOLVE_*), linear_iterations, factor [nc+1, nc] on the Cholesky paths when asked)"""
+        S = np.ascontiguousarray(S, np.float64); rhs = np.ascontiguousarray(rhs, np.float64)
+        nc = len(rhs)
+        if S.shape != (nc, nc):
+            raise ValueError("S must be [nc, nc] for rhs of length nc")
+        x = np.zeros(nc); fac = np.full((nc + 1, nc), np.nan) if factor else None
+        status = C.c_int(); iters = C.c_int()
+        _capi.check(self.lib.pxr_ba_debug_reduced_solve(self.handle, _p(S), _p(rhs), _p(x), _p(fac), C.byref(status),
+                                                        C.byref(iters)))
+        out = dict(x=x, status=status.value, linear_iterations=iters.value)
+        if factor:
+            out["factor"] = fac
+        return out
+
     def debug_inner_iterations(self):
         _capi.check(self.lib.pxr_ba_debug_inner_iterations(self.handle))
 

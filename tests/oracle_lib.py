@@ -99,6 +99,20 @@ def ba_layout(prob):
     return nc.value, nl.value, pose_off, intr_off, point_off
 
 
+PCG_STOP_ZETA, PCG_STOP_NONPOSITIVE_CURVATURE, PCG_STOP_MAX_ITERATIONS, PCG_STOP_FAILURE = range(4)
+
+
+def schur_jacobi_pcg(S, b, blk_off, blk_dim, max_iter, eta=0.1):
+    """SchurJacobiPCG (orc_ba.h) on S x = b, S symmetric [n, n] -> (x, iterations, stop reason PCG_STOP_*, ok)"""
+    S = np.ascontiguousarray(S, np.float64); b = np.ascontiguousarray(b, np.float64)
+    blk_off = np.ascontiguousarray(blk_off, np.int32); blk_dim = np.ascontiguousarray(blk_dim, np.int32)
+    n = len(b)
+    x = np.zeros(n); it = C.c_int(); stop = C.c_int()
+    rc = lib().orc_schur_jacobi_pcg(n, p(S), p(b), len(blk_off), p(blk_off), p(blk_dim), int(max_iter), C.c_double(eta),
+                                    p(x), C.byref(it), C.byref(stop))
+    return x, it.value, stop.value, rc == 0
+
+
 def ba_linearize(prob, interp, opts, radius=1e4):
     d = prob.desc()
     nc, nl, _, _, _ = ba_layout(prob)
