@@ -634,6 +634,76 @@ int pxr_qba_plan_waves(const pxr_qba_desc* desc, int32_t* wave_begin, int32_t* n
 int pxr_qba_debug_linearize(pxr_ctx* ctx, const pxr_qba_desc* desc, const pxr_interp_config* interp,
                             const pxr_solver_options* opt, double* cost, double* H, double* g, double* xy, double* rec);
 
+/* ---- batched query keypoint adjustment ------------------------------------------
+ * replaces a loop of _localization.QueryKeypointOptimizer.run: N independent queries, each one problem of pxr_ka_run's
+ * query mode (every residual block = one keypoint against one fixed descriptor).  One CTA solves one query; the
+ * keypoints written back are those pxr_ka_run writes for that query alone. */
+typedef struct {
+  int32_t n_queries;
+  /* per query */
+  const int64_t* kp_begin;        /* [n_queries+1] non-decreasing: query q owns keypoints [kp_begin[q], kp_begin[q+1]) */
+  const void* const* patch_blocks;   /* [n_queries] [patch_counts[q]][ph][pw][channels], host OR device memory */
+  const int64_t* patch_counts;       /* [n_queries] */
+  const uint8_t* patches_are_sparse; /* [n_queries] FeatureMap::IsSparse() */
+  /* per keypoint */
+  double* keypoints;              /* [n_kp][2] in/out */
+  const int64_t* kp_patch;        /* [n_kp] patch index within its query's block */
+  const int64_t* desc_begin;      /* [n_kp+1] non-decreasing: keypoint k has one residual block per descriptor in
+                                     [desc_begin[k], desc_begin[k+1]) */
+  const double* descs;            /* [desc_begin[n_kp]][channels] fixed fp64 descriptors */
+  const int32_t* corner;          /* [sum patch_counts][2], query blocks back to back */
+  const double* scale;            /* [sum patch_counts][2] */
+  double upsampling_factor;
+  double bound;                   /* KeypointOptimizerOptions::bound */
+  int32_t ph, pw, channels, patch_dtype;
+  /* bytes a wave may upload (patch blocks, host or device, descriptors and per-query state); 0: half of the free device
+   * memory at the call */
+  double max_wave_bytes;
+} pxr_qka_desc;
+
+typedef struct {
+  int32_t status;                 /* PXR_OK, or PXR_ERR_NUMERIC: initial cost not finite (the keypoints are still written
+                                     back as pxr_ka_run writes them: projected onto their bounds, not moved) */
+  int32_t num_residual_blocks;    /* 0: not solved, keypoints untouched */
+  double initial_cost;
+  double final_cost;
+  int32_t num_successful_steps;
+  int32_t num_unsuccessful_steps;
+  int32_t num_iterations;
+  int32_t termination_type;       /* as pxr_summary */
+} pxr_qka_result;
+
+/* Solves every query and writes the refined keypoints back into desc->keypoints.  results [n_queries]; n_waves and
+ * total (summed costs / steps, h2d_bytes, kernel launches, times, message) may be NULL.  Supported (dtype, channels):
+ * those of pxr_ka_run's query mode (fp16 8/16/32/64/128, fp32 and fp64 16/128); use_float_simd is
+ * PXR_ERR_UNSUPPORTED before anything is touched.  Queries are packed in order into waves of at most max_wave_bytes
+ * uploaded bytes (a larger query gets a wave of its own; a wave also ends where the queries' box constraint changes,
+ * i.e. between a sparse and a dense map when bound <= 0); device patch blocks are copied into the wave's slab and
+ * count toward its bytes.  The next wave's upload runs while the current one solves (two wave buffers when both fit
+ * in free device memory, else one), and the interrupt callback is polled between waves.
+ * Arguments are checked before the context: a NULL or malformed desc is reported without a device. */
+int pxr_qka_run(pxr_ctx* ctx, const pxr_qka_desc* desc, const pxr_interp_config* interp, const pxr_solver_options* opt,
+                pxr_qka_result* results, int32_t* n_waves, pxr_summary* total);
+
+/* ---- nearest candidate descriptor ------------------------------------------------
+ * replaces FindNearestReferences (localization/src/nearest_references.h:20-53) and the descriptor test of
+ * find_feature_inliers for many queries at once: item i is the descriptor of patch item_patch[i] of query
+ * item_query[i]'s block at image point xy[i] (the K1 interpolation of pxr_interpolate_descriptors, bit for bit),
+ * compared with the candidate rows [cand_begin[i], cand_end[i]) of cand [n_cand][channels] (fp64); items may share
+ * rows (a table of every 3D point's stored observations, uploaded once, serves every query).
+ *  best [n_items]     the first candidate row with the smallest squared L2 distance (fp64, fixed order; a NaN
+ *                     distance counts as smallest, as numpy's argmin), -1 when the range is empty
+ *  d_min [n_items]    that distance (+inf for an empty range); may be NULL
+ *  out_desc [n_items][channels] the interpolated descriptors; may be NULL
+ * patch blocks, corner and scale as in pxr_qba_desc; cand_on_device = 1 reads cand in place in device memory. */
+int pxr_query_match_run(pxr_ctx* ctx, int32_t n_queries, const void* const* patch_blocks, const int64_t* patch_counts,
+                        const int32_t* corner, const double* scale, double upsampling_factor, int32_t ph, int32_t pw,
+                        int32_t channels, int32_t patch_dtype, int64_t n_items, const int32_t* item_query,
+                        const int64_t* item_patch, const double* xy, const int64_t* cand_begin,
+                        const int64_t* cand_end, const double* cand,
+                        int64_t n_cand, int32_t cand_on_device, const pxr_interp_config* interp, int64_t* best,
+                        double* d_min, double* out_desc);
+
 /* ---- host-side integer algorithms (bit-exact targets) -------------------
  * replace _base.compute_track_labels / compute_score_labels / compute_root_labels
  * (base/src/graph.cc:126-256) and keypoint_adjustment/main.py:13-57 find_problem_labels. */

@@ -159,6 +159,35 @@ py::dict summary_dict(const pxr_summary& s, const std::vector<pxr_iteration_summ
                   "iterations"_a = iterations);
 }
 
+struct Blocks {
+  std::vector<const void*> ptrs;
+  std::vector<int64_t> counts;
+  int32_t dtype = PXR_F16, ph = 1, pw = 1, channels = 8;
+};
+
+// `patch_blocks`: one host [n_q,H,W,C] array per query, one dtype and patch shape
+Blocks patch_blocks(Fields& f, int64_t n_queries) {
+  if (!f.d.contains("patch_blocks")) throw py::value_error("missing field 'patch_blocks'");
+  py::list blocks = f.d["patch_blocks"];
+  if ((int64_t)py::len(blocks) != n_queries) throw py::value_error("one patch block per query is required");
+  Blocks b;
+  for (auto item : blocks) {
+    py::array a = py::array::ensure(item);
+    if (!a || a.ndim() != 4 || !(a.flags() & py::array::c_style))
+      throw py::value_error("patch blocks must be C-contiguous [N,H,W,C] arrays");
+    f.keep.push_back(a);
+    if (b.ptrs.empty()) {
+      b.dtype = dtype_id(a);
+      b.ph = (int32_t)a.shape(1); b.pw = (int32_t)a.shape(2); b.channels = (int32_t)a.shape(3);
+    } else if (dtype_id(a) != b.dtype || a.shape(1) != b.ph || a.shape(2) != b.pw || a.shape(3) != b.channels) {
+      throw py::value_error("patch blocks must share one dtype and patch shape");
+    }
+    b.ptrs.push_back(a.data());
+    b.counts.push_back((int64_t)a.shape(0));
+  }
+  return b;
+}
+
 struct Context {
   pxr_ctx* h = nullptr;
   explicit Context(int device) { check(pxr_ctx_create(device, &h)); }
@@ -333,25 +362,10 @@ PYBIND11_MODULE(_pxr_pybind, m) {
     d.xyz = f.arr<double>("xyz", false);
     d.obs_patch = f.arr<int64_t>("obs_patch", false);
     d.refs = f.arr<double>("refs", false);
-    if (!problem.contains("patch_blocks")) throw py::value_error("missing field 'patch_blocks'");
-    py::list blocks = problem["patch_blocks"];
-    if ((int64_t)py::len(blocks) != d.n_queries) throw py::value_error("one patch block per query is required");
-    std::vector<const void*> ptrs;
-    std::vector<int64_t> counts;
-    for (auto item : blocks) {
-      py::array a = py::array::ensure(item);
-      if (!a || a.ndim() != 4 || !(a.flags() & py::array::c_style))
-        throw py::value_error("patch blocks must be C-contiguous [N,H,W,C] arrays");
-      f.keep.push_back(a);
-      if (ptrs.empty()) {
-        d.patch_dtype = dtype_id(a);
-        d.ph = (int32_t)a.shape(1); d.pw = (int32_t)a.shape(2); d.channels = (int32_t)a.shape(3);
-      } else if (dtype_id(a) != d.patch_dtype || a.shape(1) != d.ph || a.shape(2) != d.pw || a.shape(3) != d.channels) {
-        throw py::value_error("patch blocks must share one dtype and patch shape");
-      }
-      ptrs.push_back(a.data());
-      counts.push_back((int64_t)a.shape(0));
-    }
+    Blocks pb = patch_blocks(f, d.n_queries);
+    d.patch_dtype = pb.dtype; d.ph = pb.ph; d.pw = pb.pw; d.channels = pb.channels;
+    std::vector<const void*>& ptrs = pb.ptrs;
+    std::vector<int64_t>& counts = pb.counts;
     d.patch_blocks = ptrs.data();
     d.patch_counts = counts.data();
     d.corner = f.arr<int32_t>("corner", false);
@@ -378,6 +392,85 @@ PYBIND11_MODULE(_pxr_pybind, m) {
     return py::dict("results"_a = out, "n_waves"_a = n_waves, "h2d_bytes"_a = s.h2d_bytes, "solve_time_s"_a = s.solve_time_s,
                     "total_time_s"_a = s.total_time_s);
   }, "ctx"_a, "problem"_a, "interpolation"_a = py::dict(), "options"_a = py::dict());
+  // batched query KA (a loop of QueryKeypointOptimizer.run): per query kp_begin [nq+1], patches_are_sparse [nq] and
+  // one host patch block (`patch_blocks`, `corner` / `scale` back to back); per keypoint keypoints [n,2] (refined IN
+  // PLACE), kp_patch (within its query's block) and desc_begin [n+1] into descs [m, C]
+  m.def("qka_run", [](Context& ctx, py::dict problem, py::dict interpolation, py::dict options) {
+    Fields f{problem, {}};
+    pxr_qka_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.kp_begin = f.arr<int64_t>("kp_begin");
+    d.n_queries = (int32_t)(f.len("kp_begin") - 1);
+    if (d.n_queries < 0) throw py::value_error("kp_begin must hold n_queries + 1 entries");
+    Blocks pb = patch_blocks(f, d.n_queries);
+    d.patch_dtype = pb.dtype; d.ph = pb.ph; d.pw = pb.pw; d.channels = pb.channels;
+    d.patch_blocks = pb.ptrs.data(); d.patch_counts = pb.counts.data();
+    d.patches_are_sparse = f.arr<uint8_t>("patches_are_sparse", d.n_queries > 0);
+    if (f.len("patches_are_sparse") != d.n_queries) throw py::value_error("one patches_are_sparse flag per query");
+    d.keypoints = f.inout<double>("keypoints");
+    d.kp_patch = f.arr<int64_t>("kp_patch", false);
+    d.desc_begin = f.arr<int64_t>("desc_begin", false);
+    const int64_t n_kp = f.len("keypoints");
+    if (f.len("kp_patch") != n_kp || f.len("desc_begin") != (n_kp ? n_kp + 1 : f.len("desc_begin")))
+      throw py::value_error("kp_patch must hold one entry per keypoint and desc_begin n_keypoints + 1");
+    d.descs = f.arr<double>("descs", false);
+    d.corner = f.arr<int32_t>("corner", false);
+    d.scale = f.arr<double>("scale", false);
+    d.upsampling_factor = f.scalar<double>("upsampling_factor", 1.0);
+    d.bound = f.scalar<double>("bound", 4.0);
+    d.max_wave_bytes = f.scalar<double>("max_wave_bytes", 0.0);
+    const pxr_interp_config ic = interp_config(interpolation);
+    pxr_solver_options so; pxr_default_ka_options(&so); apply_options(so, options);
+    std::vector<pxr_qka_result> res((size_t)std::max(d.n_queries, 1));
+    int32_t n_waves = 0;
+    pxr_summary s; std::memset(&s, 0, sizeof(s));
+    int rc;
+    { py::gil_scoped_release nogil; rc = pxr_qka_run(ctx.h, &d, &ic, &so, res.data(), &n_waves, &s); }
+    check(rc);
+    py::list out;
+    for (int q = 0; q < d.n_queries; ++q) {
+      const pxr_qka_result& r = res[q];
+      out.append(py::dict("status"_a = r.status, "num_residual_blocks"_a = r.num_residual_blocks,
+                          "initial_cost"_a = r.initial_cost, "final_cost"_a = r.final_cost,
+                          "num_iterations"_a = r.num_iterations, "num_successful_steps"_a = r.num_successful_steps,
+                          "num_unsuccessful_steps"_a = r.num_unsuccessful_steps, "termination_type"_a = r.termination_type));
+    }
+    return py::dict("results"_a = out, "n_waves"_a = n_waves, "h2d_bytes"_a = s.h2d_bytes, "solve_time_s"_a = s.solve_time_s,
+                    "total_time_s"_a = s.total_time_s);
+  }, "ctx"_a, "problem"_a, "interpolation"_a = py::dict(), "options"_a = py::dict());
+  // nearest candidate descriptor (FindNearestReferences for many queries): `patch_blocks` / `corner` / `scale` as in
+  // qka_run; per item item_query, item_patch, xy [n,2] and the candidate rows [cand_begin, cand_end) of cand [m, C]
+  // (host) -> dict(best, d_min, desc)
+  m.def("query_match_run", [](Context& ctx, py::dict problem, py::dict interpolation) {
+    Fields f{problem, {}};
+    const int64_t n_queries = f.len("patch_blocks");
+    Blocks pb = patch_blocks(f, n_queries);
+    const int64_t n = f.len("item_query");
+    const int32_t* iq = f.arr<int32_t>("item_query", false);
+    const int64_t* ip = f.arr<int64_t>("item_patch", false);
+    const double* xy = f.arr<double>("xy", false);
+    const int64_t* cb = f.arr<int64_t>("cand_begin", false);
+    const int64_t* ce = f.arr<int64_t>("cand_end", false);
+    if (f.len("item_patch") != n || f.len("xy") != n || f.len("cand_begin") != n || f.len("cand_end") != n)
+      throw py::value_error("one item_patch, xy, cand_begin and cand_end per item");
+    const double* cand = f.arr<double>("cand", false);
+    const int64_t n_cand = f.len("cand");
+    if (n_cand && carray<double>::ensure(problem["cand"]).size() != n_cand * pb.channels)
+      throw py::value_error("cand must be [n, channels]");
+    const int32_t* corner = f.arr<int32_t>("corner", false);
+    const double* scale = f.arr<double>("scale", false);
+    const pxr_interp_config ic = interp_config(interpolation);
+    carray<int64_t> best(n);
+    carray<double> dmin(n), desc({(py::ssize_t)n, (py::ssize_t)pb.channels});
+    int rc;
+    {
+      py::gil_scoped_release nogil;
+      rc = pxr_query_match_run(ctx.h, (int32_t)n_queries, pb.ptrs.data(), pb.counts.data(), corner, scale, 1.0, pb.ph, pb.pw, pb.channels, pb.dtype, n, iq, ip, xy, cb, ce,
+                               cand, n_cand, 0, &ic, best.mutable_data(), dmin.mutable_data(), desc.mutable_data());
+    }
+    check(rc);
+    return py::dict("best"_a = best, "d_min"_a = dmin, "desc"_a = desc);
+  }, "ctx"_a, "problem"_a, "interpolation"_a = py::dict());
   m.def("refs_compute", [](Context& ctx, py::dict problem, py::dict interpolation, int loss_type, double loss_scale, int iters) {
     Fields f{problem, {}};
     pxr_ba_desc d = ba_desc(f);

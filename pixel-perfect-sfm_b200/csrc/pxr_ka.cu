@@ -16,6 +16,7 @@
 // set (<= 50 windows x 4 KiB) is cache resident, so KA is compute/L2 bound, not HBM bound.
 #include <algorithm>
 #include <chrono>
+#include <cmath>
 #include <cstring>
 #include <unordered_map>
 #include <vector>
@@ -23,6 +24,7 @@
 #include "pxr_fm_eval.cuh"
 #include "pxr_internal.h"
 #include "pxr_lm.cuh"
+#include "pxr_waves.h"
 
 namespace pxr {
 
@@ -644,31 +646,51 @@ static int launch_ka(pxr_ctx* ctx, bool fs, bool ref, const KAArgs& a, size_t sm
   return PXR_OK;
 }
 
-}  // namespace pxr
 
-using namespace pxr;
+// the (dtype, channels) pairs of the PXR_KA_CASE dispatch
+static bool ka_supported(int dtype, int C) {
+  return (dtype == PXR_F16 && (C == 128 || C == 64 || C == 32 || C == 16 || C == 8)) ||
+         (dtype == PXR_F32 && (C == 128 || C == 16)) || (dtype == PXR_F64 && (C == 128 || C == 16));
+}
 
-extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_config* interp_in,
-                          const pxr_solver_options* opt_in, pxr_summary* summary) {
-  const auto t0 = std::chrono::steady_clock::now();
-  if (!ctx || !d) return fail(PXR_ERR_INVALID_ARGUMENT, "NULL argument");
-  if (d->n_keypoints < 0 || d->n_edges < 0 || !d->keypoints || !d->kp_const || (d->n_edges && (!d->edge_src || !d->edge_dst)) ||
-      (!d->patches && d->n_patch_blocks <= 0) || !d->corner || !d->scale || d->n_problems < 0)
-    return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
-  pxr_interp_config ic; if (interp_in) ic = *interp_in; else pxr_default_interp_config(&ic);
-  pxr_solver_options so; if (opt_in) so = *opt_in; else pxr_default_ka_options(&so);
-  const bool refmode = d->ref_desc != nullptr;
-  if (refmode && d->n_ref_desc <= 0) return fail(PXR_ERR_INVALID_ARGUMENT, "ref_desc without n_ref_desc");
-  const int C = d->channels;
-  const bool c_ok = (d->patch_dtype == PXR_F16 && (C == 128 || C == 64 || C == 32 || C == 16 || C == 8)) ||
-                    (d->patch_dtype == PXR_F32 && (C == 128 || C == 16)) || (d->patch_dtype == PXR_F64 && (C == 128 || C == 16));
-  if (!c_ok) return fail(PXR_ERR_UNSUPPORTED, "Unsupported dimensions (CHANNELS=%d, dtype=%d, N_NODES=1).", C, d->patch_dtype);
-  PXR_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t s = ctx->stream;
-  const int64_t launches0 = ctx->launches;
+// A buffer that only grows: the batched solve reuses its wave buffers across waves.  A wave larger than every earlier one
+// on the same buffer set still reallocates, and that cudaFree / cudaMalloc waits for the wave in flight.
+template <typename T>
+static int grow(DevBuf<T>& b, size_t count) { return (b.p && b.n >= count) ? (int)PXR_OK : b.alloc(count); }
+template <typename T>
+static int put(DevBuf<T>& b, const T* host, size_t count, cudaStream_t s) {
+  PXR_TRY(grow(b, count));
+  if (count) PXR_CUDA(cudaMemcpyAsync(b.p, host, count * sizeof(T), cudaMemcpyHostToDevice, s));
+  return PXR_OK;
+}
+
+// One pxr_ka_desc on the device: the host-side problem structure, its uploads and the kernel arguments.  pxr_ka_run
+// solves one; pxr_qka_run solves one per wave of queries (a query is one problem), so both make the same decisions.
+struct KASolve {
+  int P = 0, n_offchip = 0;
+  double h2d = 0;
+  std::vector<int64_t> peb, var_kp, wso;
+  std::vector<int32_t> pvb, ev1, ev2, vblo, vbhi, vboff;
+  std::vector<double> vlo, vhi;
+  DevBuf<int64_t> d_peb, d_k1, d_k2, d_varkp, d_kppatch, d_wsoff;
+  DevBuf<int32_t> d_pvb, d_v1, d_v2, d_corner, d_vblo, d_vbhi, d_vboff;
+  DevBuf<double> d_w, d_lo, d_hi, d_kp, d_scale, d_out, d_ref, d_ws;
+  DevBuf<uint8_t> d_patches;
+  KAArgs a;
+  size_t smem = 0;
+};
+
+// Host set-up of every problem of `d` (reference: TopologicalKeypointOptimizer::SetUp + ParameterizeKeypoints) and the
+// uploads, enqueued on stream s.  d->ref_desc != NULL selects query mode.
+static int ka_prepare(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_config& ic, const pxr_solver_options& so,
+                      cudaStream_t s, KASolve& k) {
   const int P = std::max(1, d->n_problems);
+  k.P = P;
+  const bool refmode = d->ref_desc != nullptr;
+  const int C = d->channels;
   // ---- host-side problem structure (reference: TopologicalKeypointOptimizer::SetUp + ParameterizeKeypoints)
-  std::vector<int64_t> peb(P + 1, 0);
+  std::vector<int64_t>& peb = k.peb;
+  peb.assign(P + 1, 0);
   for (int64_t e = 0; e < d->n_edges; ++e) {
     const int pl = d->edge_problem ? d->edge_problem[e] : 0;
     if (pl < 0 || pl >= P) return fail(PXR_ERR_INVALID_ARGUMENT, "edge_problem out of range");
@@ -679,15 +701,18 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
     peb[pl + 1]++;
   }
   for (int p = 0; p < P; ++p) peb[p + 1] += peb[p];
-  std::vector<int32_t> pvb(P + 1, 0), ev1(d->n_edges), ev2(d->n_edges);
-  std::vector<int64_t> var_kp;
-  std::vector<double> vlo, vhi;
+  std::vector<int32_t>& pvb = k.pvb; std::vector<int32_t>& ev1 = k.ev1; std::vector<int32_t>& ev2 = k.ev2;
+  std::vector<int64_t>& var_kp = k.var_kp;
+  std::vector<double>& vlo = k.vlo; std::vector<double>& vhi = k.vhi;
+  pvb.assign(P + 1, 0); ev1.assign(d->n_edges, 0); ev2.assign(d->n_edges, 0);
+  var_kp.clear(); vlo.clear(); vhi.clear();
   const bool constrained = d->bound > 0.0 || d->patches_are_sparse;
   int max_comp = 0;                     // variable keypoints of the largest component (dense mode)
   std::vector<int64_t> owner(d->n_keypoints, -1);
   // per variable: scalar range of its connected component and the offset of the component's packed triangle in the
   // problem's matrices (dense mode); per problem: doubles per matrix
-  std::vector<int32_t> vblo, vbhi, vboff;
+  std::vector<int32_t>& vblo = k.vblo; std::vector<int32_t>& vbhi = k.vbhi; std::vector<int32_t>& vboff = k.vboff;
+  vblo.clear(); vbhi.clear(); vboff.clear();
   std::vector<int64_t> pm(P, 0);
   for (int p = 0; p < P; ++p) {
     std::unordered_map<int64_t, int> idx;
@@ -763,34 +788,32 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
   // its workspace in global memory (query mode: every problem, its size is not bounded)
   int smem_optin = 0;
   PXR_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-  std::vector<int64_t> wso(P, -1);
+  std::vector<int64_t>& wso = k.wso;
+  wso.assign(P, -1);
   int64_t ws_words = 0, smem_words = 0;
-  int n_offchip = 0;
+  int& n_offchip = k.n_offchip;
+  n_offchip = 0;
   for (int p = 0; p < P; ++p) {
     const int64_t words = 2 * pm[p] + 10 * 2 * (int64_t)(pvb[p + 1] - pvb[p]);
     if (!refmode && (kKAWarps + C_N + words) * (int64_t)sizeof(double) <= smem_optin) smem_words = std::max(smem_words, words);
     else { wso[p] = ws_words; ws_words += words; ++n_offchip; }
   }
   // ---- upload
-  DevBuf<int64_t> d_peb, d_k1, d_k2, d_varkp, d_kppatch;
-  DevBuf<int32_t> d_pvb, d_v1, d_v2, d_corner;
-  DevBuf<double> d_w, d_lo, d_hi, d_kp, d_scale, d_out;
-  DevBuf<uint8_t> d_patches;
-  double h2d = 0;
-  PXR_TRY(d_peb.upload(peb.data(), peb.size(), s)); PXR_TRY(d_pvb.upload(pvb.data(), pvb.size(), s));
-  PXR_TRY(d_k1.upload(d->edge_src, d->n_edges, s)); PXR_TRY(d_k2.upload(d->edge_dst, d->n_edges, s));
-  PXR_TRY(d_v1.upload(ev1.data(), ev1.size(), s)); PXR_TRY(d_v2.upload(ev2.data(), ev2.size(), s));
-  if (d->edge_weight) PXR_TRY(d_w.upload(d->edge_weight, d->n_edges, s));
-  PXR_TRY(d_varkp.upload(var_kp.data(), var_kp.size(), s));
-  PXR_TRY(d_lo.upload(vlo.data(), vlo.size(), s)); PXR_TRY(d_hi.upload(vhi.data(), vhi.size(), s));
-  DevBuf<int32_t> d_vblo, d_vbhi, d_vboff;
-  PXR_TRY(d_vblo.upload(vblo.data(), vblo.size(), s)); PXR_TRY(d_vbhi.upload(vbhi.data(), vbhi.size(), s));
-  PXR_TRY(d_vboff.upload(vboff.data(), vboff.size(), s));
-  PXR_TRY(d_kp.upload(d->keypoints, (size_t)d->n_keypoints * 2, s));
-  if (d->kp_patch) PXR_TRY(d_kppatch.upload(d->kp_patch, d->n_keypoints, s));
+  double& h2d = k.h2d;
+  h2d = 0;
+  PXR_TRY(put(k.d_peb, peb.data(), peb.size(), s)); PXR_TRY(put(k.d_pvb, pvb.data(), pvb.size(), s));
+  PXR_TRY(put(k.d_k1, d->edge_src, d->n_edges, s)); PXR_TRY(put(k.d_k2, d->edge_dst, d->n_edges, s));
+  PXR_TRY(put(k.d_v1, ev1.data(), ev1.size(), s)); PXR_TRY(put(k.d_v2, ev2.data(), ev2.size(), s));
+  if (d->edge_weight) PXR_TRY(put(k.d_w, d->edge_weight, d->n_edges, s));
+  PXR_TRY(put(k.d_varkp, var_kp.data(), var_kp.size(), s));
+  PXR_TRY(put(k.d_lo, vlo.data(), vlo.size(), s)); PXR_TRY(put(k.d_hi, vhi.data(), vhi.size(), s));
+  PXR_TRY(put(k.d_vblo, vblo.data(), vblo.size(), s)); PXR_TRY(put(k.d_vbhi, vbhi.data(), vbhi.size(), s));
+  PXR_TRY(put(k.d_vboff, vboff.data(), vboff.size(), s));
+  PXR_TRY(put(k.d_kp, d->keypoints, (size_t)d->n_keypoints * 2, s));
+  if (d->kp_patch) PXR_TRY(put(k.d_kppatch, d->kp_patch, d->n_keypoints, s));
   const int64_t n_patches = d->kp_patch ? d->n_patches : std::max(d->n_patches, d->n_keypoints);
-  PXR_TRY(d_corner.upload(d->corner, (size_t)n_patches * 2, s)); PXR_TRY(d_scale.upload(d->scale, (size_t)n_patches * 2, s));
-  PXR_TRY(d_out.alloc((size_t)P * 6));
+  PXR_TRY(put(k.d_corner, d->corner, (size_t)n_patches * 2, s)); PXR_TRY(put(k.d_scale, d->scale, (size_t)n_patches * 2, s));
+  PXR_TRY(grow(k.d_out, (size_t)P * 6));
   const size_t esz = d->patch_dtype == PXR_F16 ? 2 : (d->patch_dtype == PXR_F32 ? 4 : 8);
   const size_t pbytes = (size_t)n_patches * d->ph * d->pw * C * esz;
   const uint8_t* dp = nullptr;
@@ -800,74 +823,316 @@ extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_c
     for (int b = 0; b < d->n_patch_blocks; ++b) tot += d->patch_block_counts[b];
     if (tot < n_patches) return fail(PXR_ERR_INVALID_ARGUMENT, "patch blocks hold %lld patches, %lld needed", (long long)tot, (long long)n_patches);
     const size_t per = (size_t)d->ph * d->pw * C * esz;
-    PXR_TRY(d_patches.alloc((size_t)tot * per));
+    PXR_TRY(grow(k.d_patches, (size_t)tot * per));
     std::vector<size_t> seg_bytes((size_t)d->n_patch_blocks);
     for (int b = 0; b < d->n_patch_blocks; ++b) seg_bytes[b] = (size_t)d->patch_block_counts[b] * per;
-    PXR_TRY(upload_segments(ctx, d_patches.p, d->patch_block_ptrs, seg_bytes.data(), d->n_patch_blocks, &h2d));
-    dp = d_patches.p;
+    PXR_TRY(upload_segments(ctx, k.d_patches.p, d->patch_block_ptrs, seg_bytes.data(), d->n_patch_blocks, &h2d, s));
+    dp = k.d_patches.p;
   } else if (d->patches_on_device) dp = (const uint8_t*)d->patches;
-  else { PXR_TRY(d_patches.alloc(pbytes)); PXR_TRY(upload_bytes(ctx, d_patches.p, d->patches, pbytes)); dp = d_patches.p; h2d += pbytes; }
+  else { PXR_TRY(grow(k.d_patches, pbytes)); PXR_TRY(upload_bytes(ctx, k.d_patches.p, d->patches, pbytes, nullptr, s)); dp = k.d_patches.p; h2d += pbytes; }
   h2d += d->n_edges * 40.0 + d->n_keypoints * 24.0;
-  KAArgs a;
-  a.n_problems = P; a.prob_edge_begin = d_peb.p; a.prob_var_begin = d_pvb.p;
-  a.e_k1 = d_k1.p; a.e_k2 = d_k2.p; a.e_v1 = d_v1.p; a.e_v2 = d_v2.p; a.e_w = d->edge_weight ? d_w.p : nullptr;
-  a.var_kp = d_varkp.p; a.var_lower = d_lo.p; a.var_upper = d_hi.p;
-  a.var_blk_lo = d_vblo.p; a.var_blk_hi = d_vbhi.p; a.var_blk_off = d_vboff.p;
-  a.keypoints = d_kp.p; a.kp_patch = d->kp_patch ? d_kppatch.p : nullptr;
-  a.patches = dp; a.ph = d->ph; a.pw = d->pw; a.corner = d_corner.p; a.scale = d_scale.p; a.ups = d->upsampling_factor;
+  KAArgs& a = k.a;
+  a.n_problems = P; a.prob_edge_begin = k.d_peb.p; a.prob_var_begin = k.d_pvb.p;
+  a.e_k1 = k.d_k1.p; a.e_k2 = k.d_k2.p; a.e_v1 = k.d_v1.p; a.e_v2 = k.d_v2.p; a.e_w = d->edge_weight ? k.d_w.p : nullptr;
+  a.var_kp = k.d_varkp.p; a.var_lower = k.d_lo.p; a.var_upper = k.d_hi.p;
+  a.var_blk_lo = k.d_vblo.p; a.var_blk_hi = k.d_vbhi.p; a.var_blk_off = k.d_vboff.p;
+  a.keypoints = k.d_kp.p; a.kp_patch = d->kp_patch ? k.d_kppatch.p : nullptr;
+  a.patches = dp; a.ph = d->ph; a.pw = d->pw; a.corner = k.d_corner.p; a.scale = k.d_scale.p; a.ups = d->upsampling_factor;
   a.loss.type = so.loss_type; a.loss.a = so.loss_scale; a.l2_normalize = ic.l2_normalize; a.constrained = constrained ? 1 : 0;
   a.max_iter = so.max_num_iterations; a.max_invalid = so.max_num_consecutive_invalid_steps;
   a.ftol = so.function_tolerance; a.gtol = so.gradient_tolerance; a.ptol = so.parameter_tolerance;
   a.min_rel_dec = so.min_relative_decrease; a.radius0 = so.initial_trust_region_radius; a.max_radius = so.max_trust_region_radius;
   a.min_radius = so.min_trust_region_radius; a.min_diag = so.min_lm_diagonal; a.max_diag = so.max_lm_diagonal;
-  a.jacobi_scaling = so.jacobi_scaling; a.prob_out = d_out.p;
+  a.jacobi_scaling = so.jacobi_scaling; a.prob_out = k.d_out.p;
   a.max_nonmonotonic = so.use_nonmonotonic_steps ? std::max(0, so.max_consecutive_nonmonotonic_steps) : 0;
-  DevBuf<double> d_ref, d_ws;
-  DevBuf<int64_t> d_wsoff;
   a.ref_desc = nullptr; a.workspace = nullptr; a.ws_off = nullptr;
   if (refmode) {
-    PXR_TRY(d_ref.upload(d->ref_desc, (size_t)d->n_ref_desc * C, s));
-    a.ref_desc = d_ref.p;
+    PXR_TRY(put(k.d_ref, d->ref_desc, (size_t)d->n_ref_desc * C, s));
+    a.ref_desc = k.d_ref.p;
     h2d += (double)d->n_ref_desc * C * 8;
   }
-  if (n_offchip > 0) {      // wso lives until the synchronisation after the launch
-    PXR_TRY(d_wsoff.upload(wso.data(), wso.size(), s));
-    PXR_TRY(d_ws.alloc((size_t)std::max<int64_t>(ws_words, 1)));
-    a.workspace = d_ws.p; a.ws_off = d_wsoff.p;
+  if (n_offchip > 0) {
+    PXR_TRY(put(k.d_wsoff, wso.data(), wso.size(), s));
+    PXR_TRY(grow(k.d_ws, (size_t)std::max<int64_t>(ws_words, 1)));
+    a.workspace = k.d_ws.p; a.ws_off = k.d_wsoff.p;
   }
-  const size_t smem = (size_t)(kKAWarps + C_N + smem_words) * sizeof(double);
-  const bool fs = ic.use_float_simd != 0;
+  k.smem = (size_t)(kKAWarps + C_N + smem_words) * sizeof(double);
+  return PXR_OK;
+}
+
+// ka_solve_kernel over the prepared problems, on ctx->stream
+static int ka_launch(pxr_ctx* ctx, const pxr_ka_desc* d, bool fs, KASolve& k) {
+  const int C = d->channels;
+  const bool refmode = d->ref_desc != nullptr;
   int rc = PXR_ERR_UNSUPPORTED;
-  cudaEvent_t tev0 = nullptr, tev1 = nullptr;
-  cudaEventCreate(&tev0); cudaEventCreate(&tev1);
-  cudaEventRecord(tev0, s);
-#define PXR_KA_CASE(T, CC) if (C == CC) rc = launch_ka<T, CC>(ctx, fs, refmode, a, smem);
+#define PXR_KA_CASE(T, CC) if (C == CC) rc = launch_ka<T, CC>(ctx, fs, refmode, k.a, k.smem);
   if (d->patch_dtype == PXR_F16) { PXR_KA_CASE(__half, 128) PXR_KA_CASE(__half, 64) PXR_KA_CASE(__half, 32) PXR_KA_CASE(__half, 16) PXR_KA_CASE(__half, 8) }
   else if (d->patch_dtype == PXR_F32) { PXR_KA_CASE(float, 128) PXR_KA_CASE(float, 16) }
   else { PXR_KA_CASE(double, 128) PXR_KA_CASE(double, 16) }
 #undef PXR_KA_CASE
+  return rc;
+}
+
+}  // namespace pxr
+
+using namespace pxr;
+
+extern "C" int pxr_ka_run(pxr_ctx* ctx, const pxr_ka_desc* d, const pxr_interp_config* interp_in,
+                          const pxr_solver_options* opt_in, pxr_summary* summary) {
+  const auto t0 = std::chrono::steady_clock::now();
+  if (!ctx || !d) return fail(PXR_ERR_INVALID_ARGUMENT, "NULL argument");
+  if (d->n_keypoints < 0 || d->n_edges < 0 || !d->keypoints || !d->kp_const || (d->n_edges && (!d->edge_src || !d->edge_dst)) ||
+      (!d->patches && d->n_patch_blocks <= 0) || !d->corner || !d->scale || d->n_problems < 0)
+    return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  pxr_interp_config ic; if (interp_in) ic = *interp_in; else pxr_default_interp_config(&ic);
+  pxr_solver_options so; if (opt_in) so = *opt_in; else pxr_default_ka_options(&so);
+  const bool refmode = d->ref_desc != nullptr;
+  if (refmode && d->n_ref_desc <= 0) return fail(PXR_ERR_INVALID_ARGUMENT, "ref_desc without n_ref_desc");
+  const int C = d->channels;
+  if (!ka_supported(d->patch_dtype, C)) return fail(PXR_ERR_UNSUPPORTED, "Unsupported dimensions (CHANNELS=%d, dtype=%d, N_NODES=1).", C, d->patch_dtype);
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  const int64_t launches0 = ctx->launches;
+  KASolve k;
+  PXR_TRY(ka_prepare(ctx, d, ic, so, s, k));
+  const int P = k.P;
+  const bool fs = ic.use_float_simd != 0;
+  cudaEvent_t tev0 = nullptr, tev1 = nullptr;
+  cudaEventCreate(&tev0); cudaEventCreate(&tev1);
+  cudaEventRecord(tev0, s);
+  const int rc = ka_launch(ctx, d, fs, k);
   cudaEventRecord(tev1, s);
   if (rc != PXR_OK) { cudaEventDestroy(tev0); cudaEventDestroy(tev1); return rc; }
   std::vector<double> out((size_t)P * 6);
-  PXR_CUDA(cudaMemcpyAsync(out.data(), d_out.p, out.size() * 8, cudaMemcpyDeviceToHost, s));
-  PXR_CUDA(cudaMemcpyAsync(d->keypoints, d_kp.p, (size_t)d->n_keypoints * 16, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaMemcpyAsync(out.data(), k.d_out.p, out.size() * 8, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaMemcpyAsync(d->keypoints, k.d_kp.p, (size_t)d->n_keypoints * 16, cudaMemcpyDeviceToHost, s));
   PXR_CUDA(cudaStreamSynchronize(s));
   if (summary) {
     double ic0 = 0, fc = 0; int ns = 0, nu = 0, iters = 0;
     for (int p = 0; p < P; ++p) { ic0 += out[p * 6]; fc += out[p * 6 + 1]; iters = std::max(iters, (int)out[p * 6 + 2]); ns += (int)out[p * 6 + 3]; nu += (int)out[p * 6 + 4]; }
     summary->initial_cost = ic0; summary->final_cost = fc;
-    summary->num_residual_blocks = (int32_t)d->n_edges; summary->num_residuals = d->n_edges * C;
+    summary->num_residual_blocks = (int32_t)d->n_edges; summary->num_residuals = d->n_edges * d->channels;
     summary->num_successful_steps = ns; summary->num_unsuccessful_steps = nu; summary->num_inner_iteration_steps = 0;
     summary->termination_type = 0; summary->num_iterations = 0;
-    summary->h2d_bytes = h2d; summary->d2h_bytes = d->n_keypoints * 16.0 + P * 48.0;
+    summary->h2d_bytes = k.h2d; summary->d2h_bytes = d->n_keypoints * 16.0 + P * 48.0;
     summary->kernel_launches = ctx->launches - launches0;
     summary->solve_time_s = summary->total_time_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     float kms = 0.f;
     cudaEventElapsedTime(&kms, tev0, tev1);
     std::snprintf(summary->message, sizeof(summary->message),
                   "%d problems, max %d LM iterations, solve kernel %.3f ms, %d with an off-chip workspace", P, iters, kms,
-                  n_offchip);
+                  k.n_offchip);
   }
   cudaEventDestroy(tev0); cudaEventDestroy(tev1);
+  return PXR_OK;
+}
+
+// ---- batched query keypoint adjustment: one query = one problem of the query mode, solved wave by wave
+namespace pxr {
+
+static int check_qka(const pxr_qka_desc* d, const pxr_interp_config* ic) {
+  if (!d) return fail(PXR_ERR_INVALID_ARGUMENT, "desc is NULL");
+  if (d->n_queries < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "n_queries < 0");
+  if (d->n_queries > 0 && (!d->kp_begin || !d->patch_blocks || !d->patch_counts || !d->patches_are_sparse))
+    return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  if (ic && ic->check_bounds) return fail(PXR_ERR_UNSUPPORTED, "check_bounds=true is not supported on this path");
+  if (ic && ic->use_float_simd) return fail(PXR_ERR_UNSUPPORTED, "use_float_simd is not built for the query (reference-descriptor) mode");
+  if (!ka_supported(d->patch_dtype, d->channels))
+    return fail(PXR_ERR_UNSUPPORTED, "Unsupported dimensions (CHANNELS=%d, dtype=%d, N_NODES=1).", d->channels, d->patch_dtype);
+  if (d->ph < 1 || d->pw < 1) return fail(PXR_ERR_INVALID_ARGUMENT, "bad patch size");
+  if (!(d->upsampling_factor > 0.0)) return fail(PXR_ERR_INVALID_ARGUMENT, "upsampling_factor must be > 0");
+  if (d->n_queries == 0) return PXR_OK;
+  if (d->kp_begin[0] != 0) return fail(PXR_ERR_INVALID_ARGUMENT, "kp_begin[0] must be 0");
+  int64_t n_patches = 0;
+  for (int q = 0; q < d->n_queries; ++q) {
+    if (d->kp_begin[q + 1] < d->kp_begin[q]) return fail(PXR_ERR_INVALID_ARGUMENT, "kp_begin must be non-decreasing");
+    if (d->patch_counts[q] < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "patch_counts[%d] < 0", q);
+    if (d->patch_counts[q] > 0 && !d->patch_blocks[q]) return fail(PXR_ERR_INVALID_ARGUMENT, "patch block %d is NULL", q);
+    n_patches += d->patch_counts[q];
+  }
+  const int64_t n_kp = d->kp_begin[d->n_queries];
+  if (n_kp > 0 && (!d->keypoints || !d->kp_patch || !d->desc_begin)) return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  if (n_patches > 0 && (!d->corner || !d->scale)) return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  if (n_kp == 0) return PXR_OK;
+  if (d->desc_begin[0] != 0) return fail(PXR_ERR_INVALID_ARGUMENT, "desc_begin[0] must be 0");
+  for (int64_t k = 0; k < n_kp; ++k)
+    if (d->desc_begin[k + 1] < d->desc_begin[k]) return fail(PXR_ERR_INVALID_ARGUMENT, "desc_begin must be non-decreasing");
+  if (d->desc_begin[n_kp] > 0 && !d->descs) return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  for (int q = 0; q < d->n_queries; ++q)
+    for (int64_t k = d->kp_begin[q]; k < d->kp_begin[q + 1]; ++k)
+      if (d->kp_patch[k] < 0 || d->kp_patch[k] >= d->patch_counts[q])
+        return fail(PXR_ERR_INVALID_ARGUMENT, "kp_patch[%lld] is not a patch of query %d", (long long)k, q);
+  return PXR_OK;
+}
+
+static bool qka_constrained(const pxr_qka_desc* d, int q) { return d->bound > 0.0 || d->patches_are_sparse[q]; }
+static int64_t qka_blocks(const pxr_qka_desc* d, int q) {
+  return d->desc_begin[d->kp_begin[q + 1]] - d->desc_begin[d->kp_begin[q]];
+}
+
+// device bytes of query q in a wave: its patches (host or device: both are copied into the wave's slab), corners and
+// scales, per keypoint the keypoint, patch index, variable state and off-chip workspace (26 doubles), per residual
+// block its descriptor and edge, and the problem's offsets and outputs
+static double qka_query_bytes(const pxr_qka_desc* d, int q) {
+  const double patch = (double)d->ph * d->pw * d->channels * dtype_bytes(d->patch_dtype);
+  const double nk = (double)(d->kp_begin[q + 1] - d->kp_begin[q]);
+  return d->patch_counts[q] * (patch + 24.0) + nk * (16.0 + 8.0 + 8.0 + 32.0 + 12.0 + 26.0 * 8.0 + 1.0) +
+         (double)qka_blocks(d, q) * (d->channels * 8.0 + 24.0) + (8.0 + 4.0 + 48.0 + 8.0);
+}
+
+static void qka_plan(const pxr_qka_desc* d, double budget, WavePlan* p) {
+  plan_waves(d->n_queries, d->patch_blocks, d->patch_counts, 12.0 /* closing problem offsets */, budget,
+             [d](int q, bool) { return qka_query_bytes(d, q); }, p,
+             [d](int q) { return qka_constrained(d, q) != qka_constrained(d, q - 1); });
+}
+
+// the pxr_ka_desc of one wave: its queries as the problems of one query-mode call (host arrays kept alive here)
+struct QKAWave {
+  int q0 = 0, nq = 0;
+  int64_t k0 = 0, nk = 0, p0 = 0;
+  std::vector<int64_t> es, ed, kp_patch;
+  std::vector<int32_t> ep;
+  std::vector<uint8_t> kp_const;
+  std::vector<const void*> blocks;
+  pxr_ka_desc desc;
+};
+
+static void qka_wave(const pxr_qka_desc* d, const WavePlan& plan, int w, QKAWave& v) {
+  static const double kNoDesc = 0.0;
+  static const uint8_t kNoPatch = 0;
+  v.q0 = plan.begin[w]; v.nq = plan.begin[w + 1] - v.q0;
+  v.k0 = d->kp_begin[v.q0]; v.nk = d->kp_begin[v.q0 + v.nq] - v.k0;
+  v.p0 = 0; for (int q = 0; q < v.q0; ++q) v.p0 += d->patch_counts[q];
+  const int64_t db0 = v.nk ? d->desc_begin[v.k0] : 0;
+  v.es.clear(); v.ed.clear(); v.ep.clear(); v.kp_patch.assign((size_t)v.nk, 0); v.kp_const.assign((size_t)std::max<int64_t>(v.nk, 1), 0);
+  v.blocks.assign((size_t)v.nq, &kNoPatch);
+  int64_t poff = 0;
+  for (int i = 0; i < v.nq; ++i) {
+    const int q = v.q0 + i;
+    if (d->patch_counts[q] > 0) v.blocks[i] = d->patch_blocks[q];
+    for (int64_t k = d->kp_begin[q]; k < d->kp_begin[q + 1]; ++k) {
+      v.kp_patch[k - v.k0] = poff + d->kp_patch[k];
+      for (int64_t j = d->desc_begin[k]; j < d->desc_begin[k + 1]; ++j) { v.es.push_back(k - v.k0); v.ed.push_back(j - db0); v.ep.push_back(i); }
+    }
+    poff += d->patch_counts[q];
+  }
+  pxr_ka_desc& a = v.desc;
+  std::memset(&a, 0, sizeof(a));
+  a.n_keypoints = v.nk; a.keypoints = d->keypoints ? d->keypoints + 2 * v.k0 : nullptr; a.kp_const = v.kp_const.data();
+  a.kp_patch = v.kp_patch.data();
+  a.n_edges = (int64_t)v.es.size(); a.edge_src = v.es.data(); a.edge_dst = v.ed.data(); a.edge_weight = nullptr;
+  a.edge_problem = v.ep.data(); a.n_problems = v.nq;
+  a.n_patches = poff; a.patches = nullptr; a.patches_on_device = 0;
+  a.patch_dtype = d->patch_dtype; a.ph = d->ph; a.pw = d->pw; a.channels = d->channels;
+  a.corner = d->corner ? d->corner + 2 * v.p0 : nullptr; a.scale = d->scale ? d->scale + 2 * v.p0 : nullptr;
+  a.upsampling_factor = d->upsampling_factor; a.bound = d->bound; a.patches_are_sparse = d->patches_are_sparse[v.q0];
+  a.n_patch_blocks = v.nq; a.patch_block_ptrs = v.blocks.data(); a.patch_block_counts = d->patch_counts + v.q0;
+  a.ref_desc = (d->descs && v.nk) ? d->descs + db0 * d->channels : &kNoDesc;
+  a.n_ref_desc = v.nk ? d->desc_begin[v.k0 + v.nk] - db0 : 0;
+}
+
+}  // namespace pxr
+
+extern "C" int pxr_qka_run(pxr_ctx* ctx, const pxr_qka_desc* d, const pxr_interp_config* interp_in,
+                           const pxr_solver_options* opt_in, pxr_qka_result* results, int32_t* n_waves_out,
+                           pxr_summary* total) {
+  const auto t0 = std::chrono::steady_clock::now();
+  PXR_TRY(check_qka(d, interp_in));
+  PXR_TRY(require_ctx(ctx));
+  if (!results && d->n_queries > 0) return fail(PXR_ERR_INVALID_ARGUMENT, "results is NULL");
+  pxr_interp_config ic; if (interp_in) ic = *interp_in; else pxr_default_interp_config(&ic);
+  pxr_solver_options so; if (opt_in) so = *opt_in; else pxr_default_ka_options(&so);
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  cudaStream_t us = nullptr;
+  PXR_TRY(upload_stream(ctx, &us));
+  const int64_t launches0 = ctx->launches;
+  double budget = 0.0;
+  PXR_TRY(wave_budget(d->max_wave_bytes, &budget));
+  WavePlan plan;
+  qka_plan(d, budget, &plan);
+  const int nw = (int)plan.bytes.size();
+  double max_bytes = 0.0; int64_t max_out = 1;
+  for (int w = 0; w < nw; ++w) {
+    max_bytes = std::max(max_bytes, plan.bytes[w]);
+    const int nq = plan.begin[w + 1] - plan.begin[w];
+    const int64_t nk = d->kp_begin[plan.begin[w + 1]] - d->kp_begin[plan.begin[w]];
+    max_out = std::max<int64_t>(max_out, (int64_t)nq * 6 + nk * 2);
+  }
+  int nsets = 1;
+  PXR_TRY(wave_sets(nw, (size_t)max_bytes, &nsets));
+  KASolve ks[2];
+  QKAWave wv[2];
+  // per buffer set, the pinned host copy of a wave's outputs: per-problem results | keypoints
+  struct Pinned { void* p = nullptr; ~Pinned() { if (p) cudaFreeHost(p); } } hout[2];
+  for (int k = 0; k < nsets; ++k) PXR_CUDA(cudaMallocHost(&hout[k].p, (size_t)max_out * 8));
+  cudaEvent_t kt0 = nullptr, kt1 = nullptr;
+  struct Events { cudaEvent_t* a; cudaEvent_t* b; ~Events() { if (*a) cudaEventDestroy(*a); if (*b) cudaEventDestroy(*b); } } guard{&kt0, &kt1};
+  PXR_CUDA(cudaEventCreate(&kt0));
+  PXR_CUDA(cudaEventCreate(&kt1));
+  double h2d = 0.0, kernel_ms = 0.0, ic0 = 0.0, fc = 0.0;
+  int ns = 0, nu = 0;
+  WaveSteps steps;
+  steps.upload = [&](int w, int set) {
+    qka_wave(d, plan, w, wv[set]);
+    PXR_TRY(ka_prepare(ctx, &wv[set].desc, ic, so, us, ks[set]));
+    h2d += ks[set].h2d;
+    return (int)PXR_OK;
+  };
+  steps.launch = [&](int, int set) {
+    const QKAWave& v = wv[set];
+    PXR_CUDA(cudaEventRecord(kt0, s));
+    PXR_TRY(ka_launch(ctx, &v.desc, false, ks[set]));
+    PXR_CUDA(cudaEventRecord(kt1, s));
+    double* ho = static_cast<double*>(hout[set].p);
+    PXR_CUDA(cudaMemcpyAsync(ho, ks[set].d_out.p, (size_t)v.nq * 6 * 8, cudaMemcpyDeviceToHost, s));
+    if (v.nk) PXR_CUDA(cudaMemcpyAsync(ho + (size_t)v.nq * 6, ks[set].d_kp.p, (size_t)v.nk * 16, cudaMemcpyDeviceToHost, s));
+    return (int)PXR_OK;
+  };
+  steps.finish = [&](int w, int set) {
+    // the wave's bounds from the plan: with one buffer set wv[set] already describes the next wave
+    const int q0 = plan.begin[w], nq = plan.begin[w + 1] - q0;
+    const int64_t k0 = d->kp_begin[q0];
+    const double* ho = static_cast<const double*>(hout[set].p);
+    float ms = 0.f;
+    if (cudaEventElapsedTime(&ms, kt0, kt1) == cudaSuccess) kernel_ms += ms;
+    for (int i = 0; i < nq; ++i) {
+      const int q = q0 + i;
+      const double* o = ho + (size_t)i * 6;
+      pxr_qka_result& r = results[q];
+      r.num_residual_blocks = (int32_t)qka_blocks(d, q);
+      r.initial_cost = o[0]; r.final_cost = o[1]; r.num_iterations = (int32_t)o[2];
+      r.num_successful_steps = (int32_t)o[3]; r.num_unsuccessful_steps = (int32_t)o[4]; r.termination_type = (int32_t)o[5];
+      r.status = std::isfinite(o[0]) ? PXR_OK : PXR_ERR_NUMERIC;
+      if (r.num_residual_blocks == 0) continue;   // keypoints untouched
+      // written back whatever the status: pxr_ka_run writes what the kernel leaves for such a query too
+      const int64_t kb = d->kp_begin[q], ke = d->kp_begin[q + 1];
+      std::memcpy(d->keypoints + 2 * kb, ho + (size_t)nq * 6 + 2 * (kb - k0), (size_t)(ke - kb) * 16);
+      if (r.status != PXR_OK) continue;
+      ic0 += r.initial_cost; fc += r.final_cost; ns += r.num_successful_steps; nu += r.num_unsuccessful_steps;
+    }
+    return (int)PXR_OK;
+  };
+  int done = 0;
+  const int rc = run_waves(ctx, nw, nsets, us, steps, &done);
+  if (n_waves_out) *n_waves_out = done;
+  if (rc != PXR_OK) return rc;
+  if (total) {
+    const int cap = total->iterations_capacity;
+    pxr_iteration_summary* keep = total->iterations;
+    std::memset(total, 0, sizeof(*total));
+    total->iterations_capacity = cap; total->iterations = keep;
+    total->initial_cost = ic0; total->final_cost = fc;
+    int64_t nb = 0; for (int q = 0; q < d->n_queries; ++q) nb += qka_blocks(d, q);
+    total->num_residual_blocks = (int32_t)nb;
+    total->num_residuals = nb * d->channels;
+    total->num_successful_steps = ns; total->num_unsuccessful_steps = nu;
+    total->h2d_bytes = h2d;
+    total->kernel_launches = ctx->launches - launches0;
+    total->total_time_s = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    total->solve_time_s = kernel_ms * 1e-3;
+    std::snprintf(total->message, sizeof(total->message), "%d queries in %d waves, solve kernels %.3f ms", d->n_queries, nw,
+                  kernel_ms);
+  }
   return PXR_OK;
 }

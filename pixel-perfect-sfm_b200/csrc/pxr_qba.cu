@@ -25,6 +25,7 @@
 #include "pxr_fm_eval.cuh"
 #include "pxr_internal.h"
 #include "pxr_lm.cuh"
+#include "pxr_waves.h"
 
 namespace pxr {
 
@@ -442,14 +443,6 @@ static int launch_qba(pxr_ctx* ctx, int dtype, int C, bool fs, const QBAArgs& a,
 // ---- host side --------------------------------------------------------------------------------------------------
 constexpr double kQueryStateBytes = kQParams * 8 + 8 + 8 + 8 + 4 + 4;   // params, obs_begin, patch address, first row, model, mask
 
-static size_t dtype_bytes(int dt) { return dt == PXR_F16 ? 2 : (dt == PXR_F32 ? 4 : 8); }
-
-static bool on_device(const void* p) {
-  cudaPointerAttributes pa;
-  if (!p || cudaPointerGetAttributes(&pa, p) != cudaSuccess) { cudaGetLastError(); return false; }
-  return pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged;
-}
-
 static int check_qba(const pxr_qba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so) {
   if (!d) return fail(PXR_ERR_INVALID_ARGUMENT, "desc is NULL");
   if (d->n_queries < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "n_queries < 0");
@@ -487,20 +480,8 @@ static int check_qba(const pxr_qba_desc* d, const pxr_interp_config* ic, const p
 
 static int qba_args(pxr_ctx* ctx, const pxr_qba_desc* d, const pxr_interp_config* ic, const pxr_solver_options* so) {
   PXR_TRY(check_qba(d, ic, so));
-  if (ctx) return PXR_OK;
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    return fail(PXR_ERR_NO_DEVICE, "no CUDA device available; libpxr has no CPU fallback");
-  }
-  return fail(PXR_ERR_INVALID_ARGUMENT, "ctx is NULL");
+  return require_ctx(ctx);
 }
-
-struct WavePlan {
-  std::vector<int32_t> begin;       // [n_waves + 1]
-  std::vector<double> bytes;        // [n_waves]
-  std::vector<uint8_t> host_patch;  // [n_queries] 1: the block is uploaded
-};
 
 static double query_bytes(const pxr_qba_desc* d, int q, bool host_patch) {
   const double patch = (double)d->ph * d->pw * d->channels * dtype_bytes(d->patch_dtype);
@@ -509,31 +490,9 @@ static double query_bytes(const pxr_qba_desc* d, int q, bool host_patch) {
          d->patch_counts[q] * 16.0 + kQueryStateBytes;
 }
 
-// consecutive queries while the wave fits the budget; a query larger than the budget gets a wave of its own
 static void plan_waves(const pxr_qba_desc* d, double budget, WavePlan* p) {
-  p->begin.assign(1, 0); p->bytes.clear();
-  p->host_patch.assign((size_t)d->n_queries, 0);
-  double cur = 8.0;      // obs_begin's closing entry
-  for (int q = 0; q < d->n_queries; ++q) {
-    p->host_patch[q] = (d->patch_counts[q] > 0 && !on_device(d->patch_blocks[q])) ? 1 : 0;
-    const double b = query_bytes(d, q, p->host_patch[q] != 0);
-    if (q > p->begin.back() && cur + b > budget) { p->bytes.push_back(cur); p->begin.push_back(q); cur = 8.0; }
-    cur += b;
-  }
-  if (d->n_queries > 0) { p->bytes.push_back(cur); p->begin.push_back(d->n_queries); }
-}
-
-static int wave_budget(const pxr_qba_desc* d, double* budget) {
-  if (d->max_wave_bytes > 0.0) { *budget = d->max_wave_bytes; return PXR_OK; }
-  int count = 0;
-  if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) {
-    cudaGetLastError();
-    return fail(PXR_ERR_NO_DEVICE, "max_wave_bytes 0 means half of the free device memory, and there is no CUDA device");
-  }
-  size_t fr = 0, tot = 0;
-  PXR_CUDA(cudaMemGetInfo(&fr, &tot));
-  *budget = 0.5 * (double)fr;
-  return PXR_OK;
+  plan_waves(d->n_queries, d->patch_blocks, d->patch_counts, 8.0 /* obs_begin's closing entry */, budget,
+             [d](int q, bool host_patch) { return query_bytes(d, q, host_patch); }, p);
 }
 
 // Device memory of one wave: [host patch blocks | refs | xyz | obs_patch | corner | scale | per-query state]
@@ -668,7 +627,7 @@ extern "C" int pxr_qba_plan_waves(const pxr_qba_desc* d, int32_t* wave_begin, in
   PXR_TRY(check_qba(d, nullptr, nullptr));
   if (!wave_begin || !n_waves) return fail(PXR_ERR_INVALID_ARGUMENT, "wave_begin / n_waves is NULL");
   double budget = 0.0;
-  PXR_TRY(wave_budget(d, &budget));
+  PXR_TRY(wave_budget(d->max_wave_bytes, &budget));
   WavePlan p;
   plan_waves(d, budget, &p);
   *n_waves = (int32_t)p.bytes.size();
@@ -693,22 +652,17 @@ extern "C" int pxr_qba_run(pxr_ctx* ctx, const pxr_qba_desc* d, const pxr_interp
   PXR_TRY(upload_stream(ctx, &us));
   const int64_t launches0 = ctx->launches;
   double budget = 0.0;
-  PXR_TRY(wave_budget(d, &budget));
+  PXR_TRY(wave_budget(d->max_wave_bytes, &budget));
   WavePlan plan;
   plan_waves(d, budget, &plan);
   const int nw = (int)plan.bytes.size();
-  // two wave buffers (the next upload runs while the current wave solves) when both fit; PXR_QBA_WAVE_BUFFERS=1 keeps
-  // one (tests: the one-buffer ordering is otherwise reached only by waves near half the free memory)
   size_t max_arena = 0; int max_nq = 0;
   for (int w = 0; w < nw; ++w) {
     const WaveView v = wave_view(d, plan, w);
     max_arena = std::max(max_arena, v.end); max_nq = std::max(max_nq, v.nq);
   }
-  size_t fr = 0, tot = 0;
-  PXR_CUDA(cudaMemGetInfo(&fr, &tot));
-  const char* one_buf = std::getenv("PXR_QBA_WAVE_BUFFERS");
-  const bool force_one = one_buf && std::atoi(one_buf) == 1;
-  const int nsets = (!force_one && nw > 1 && 2.0 * (double)max_arena < 0.9 * (double)fr) ? 2 : 1;
+  int nsets = 1;
+  PXR_TRY(wave_sets(nw, max_arena, &nsets));
   WaveBufs bufs[2];
   // per buffer set, the pinned host copy of a wave's outputs: params | results | iteration summaries
   const size_t out_params = (size_t)std::max(max_nq, 1) * kQParams * 8;
@@ -721,46 +675,36 @@ extern "C" int pxr_qba_run(pxr_ctx* ctx, const pxr_qba_desc* d, const pxr_interp
     if (iterations_capacity > 0) PXR_TRY(bufs[k].iters.alloc((size_t)std::max(max_nq, 1) * iterations_capacity));
     PXR_CUDA(cudaMallocHost(&hout[k].p, out_bytes));
   }
-  cudaEvent_t up_done[2] = {nullptr, nullptr}, k_done[2] = {nullptr, nullptr}, kt0 = nullptr, kt1 = nullptr;
-  struct Events { cudaEvent_t* e; int n; ~Events() { for (int i = 0; i < n; ++i) if (e[i]) cudaEventDestroy(e[i]); } };
-  cudaEvent_t all_ev[6];
-  Events guard{all_ev, 0};
-  for (cudaEvent_t* e : {&up_done[0], &up_done[1], &k_done[0], &k_done[1]}) {
-    PXR_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-    all_ev[guard.n++] = *e;
-  }
-  PXR_CUDA(cudaEventCreate(&kt0)); all_ev[guard.n++] = kt0;
-  PXR_CUDA(cudaEventCreate(&kt1)); all_ev[guard.n++] = kt1;
+  cudaEvent_t kt0 = nullptr, kt1 = nullptr;
+  struct Events { cudaEvent_t* a; cudaEvent_t* b; ~Events() { if (*a) cudaEventDestroy(*a); if (*b) cudaEventDestroy(*b); } } guard{&kt0, &kt1};
+  PXR_CUDA(cudaEventCreate(&kt0));
+  PXR_CUDA(cudaEventCreate(&kt1));
   double h2d = 0.0, kernel_ms = 0.0;
   double ic0 = 0.0, fc = 0.0; int ns = 0, nu = 0;
-  if (nw > 0) PXR_TRY(upload_wave(ctx, d, plan, wave_view(d, plan, 0), bufs[0], us, &h2d));
-  for (int w = 0; w < nw; ++w) {
-    const int set = nsets == 2 ? (w & 1) : 0;
+  WaveSteps steps;
+  steps.upload = [&](int w, int set) { return upload_wave(ctx, d, plan, wave_view(d, plan, w), bufs[set], us, &h2d); };
+  steps.launch = [&](int w, int set) {
     const WaveView v = wave_view(d, plan, w);
     WaveBufs& b = bufs[set];
-    PXR_CUDA(cudaEventRecord(up_done[set], us));
-    PXR_CUDA(cudaStreamWaitEvent(s, up_done[set], 0));
     const QBAArgs a = make_args(d, ic, so, v, b, iterations_capacity);
     PXR_CUDA(cudaEventRecord(kt0, s));
     PXR_TRY(launch_qba(ctx, d->patch_dtype, d->channels, ic.use_float_simd != 0, a, qba_smem(a)));
     PXR_CUDA(cudaEventRecord(kt1, s));
-    // the wave's outputs leave the arena before k_done: a later upload into this arena waits for k_done
+    // the wave's outputs leave the arena before the wave is done: a later upload into this arena waits for that
     uint8_t* ho = static_cast<uint8_t*>(hout[set].p);
-    const double* params = reinterpret_cast<const double*>(ho);
-    const pxr_qba_result* wres = reinterpret_cast<const pxr_qba_result*>(ho + out_params);
-    const pxr_iteration_summary* wits = reinterpret_cast<const pxr_iteration_summary*>(ho + out_params + out_res);
     PXR_CUDA(cudaMemcpyAsync(ho, a.params, (size_t)v.nq * kQParams * 8, cudaMemcpyDeviceToHost, s));
     PXR_CUDA(cudaMemcpyAsync(ho + out_params, b.results.p, (size_t)v.nq * sizeof(pxr_qba_result), cudaMemcpyDeviceToHost, s));
     if (iterations_capacity > 0)
       PXR_CUDA(cudaMemcpyAsync(ho + out_params + out_res, b.iters.p,
                                (size_t)v.nq * iterations_capacity * sizeof(pxr_iteration_summary), cudaMemcpyDeviceToHost, s));
-    PXR_CUDA(cudaEventRecord(k_done[set], s));
-    if (w + 1 < nw) {        // the next upload goes out before the host waits for this wave
-      const int nset = nsets == 2 ? 1 - set : 0;
-      if (nsets == 1) PXR_CUDA(cudaStreamWaitEvent(us, k_done[set], 0));
-      PXR_TRY(upload_wave(ctx, d, plan, wave_view(d, plan, w + 1), bufs[nset], us, &h2d));
-    }
-    PXR_CUDA(cudaEventSynchronize(k_done[set]));
+    return (int)PXR_OK;
+  };
+  steps.finish = [&](int w, int set) {
+    const WaveView v = wave_view(d, plan, w);
+    const uint8_t* ho = static_cast<const uint8_t*>(hout[set].p);
+    const double* params = reinterpret_cast<const double*>(ho);
+    const pxr_qba_result* wres = reinterpret_cast<const pxr_qba_result*>(ho + out_params);
+    const pxr_iteration_summary* wits = reinterpret_cast<const pxr_iteration_summary*>(ho + out_params + out_res);
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, kt0, kt1) == cudaSuccess) kernel_ms += ms;
     for (int i = 0; i < v.nq; ++i) {
@@ -778,14 +722,12 @@ extern "C" int pxr_qba_run(pxr_ctx* ctx, const pxr_qba_desc* d, const pxr_interp
       std::memcpy(d->tvec + (size_t)q * 3, p + kMaxK + 4, 24);
       ic0 += r.initial_cost; fc += r.final_cost; ns += r.num_successful_steps; nu += r.num_unsuccessful_steps;
     }
-    if (w + 1 < nw && interrupt_pending()) {
-      cudaStreamSynchronize(us);
-      if (n_waves_out) *n_waves_out = w + 1;
-      return fail(PXR_ERR_INTERRUPTED, "interrupted by the host after wave %d of %d", w + 1, nw);
-    }
-  }
-  PXR_CUDA(cudaStreamSynchronize(us));
-  if (n_waves_out) *n_waves_out = nw;
+    return (int)PXR_OK;
+  };
+  int done = 0;
+  const int rc = run_waves(ctx, nw, nsets, us, steps, &done);
+  if (n_waves_out) *n_waves_out = done;
+  if (rc != PXR_OK) return rc;
   if (total) {
     const int cap = total->iterations_capacity;
     pxr_iteration_summary* keep = total->iterations;

@@ -6,7 +6,10 @@
 // (FillDescriptorTrack :300-318 -> K0 + K1 in descriptor mode), run RobustMeanIRLS
 // (pixsfm/base/src/irls_optim.h:23-71; weights 1/rho(||d_i - mu||^2), NB rho not rho') and keep
 // the observation closest to the robust mean (closest_to_robust_mean, :249-272; first minimum).
+#include <cmath>
+
 #include "pxr_ba_host.h"
+#include "pxr_waves.h"
 
 namespace pxr {
 
@@ -159,6 +162,39 @@ static int read_src(pxr_ctx* ctx, const BA& b, const DevBuf<int64_t>& src, int64
     if (src_obs_out) src_obs_out[p] = hsrc[p];
   }
   return PXR_OK;
+}
+
+// Nearest candidate (FindNearestReferences, nearest_references.h:40-47): one warp per item walks its candidate rows;
+// lanes stride the channels, each lane sums its channels in order, the lanes' partials meet in a butterfly (fixed
+// order), and the first row with the smallest distance wins (strict <; a NaN distance counts as smallest, as in
+// numpy's argmin, which the per-query path uses).  Reads C * 8 bytes per candidate once.
+constexpr int kNCMaxC = 256;
+__global__ void __launch_bounds__(256) nearest_candidate_kernel(const double* __restrict__ qd,
+                                                                const int64_t* __restrict__ cand_begin,
+                                                                const int64_t* __restrict__ cand_end,
+                                                                const double* __restrict__ cand, int64_t n_items, int C,
+                                                                int64_t* __restrict__ best, double* __restrict__ d_min) {
+  const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (i >= n_items) return;
+  double q[kNCMaxC / 32];
+#pragma unroll
+  for (int k = 0; k < kNCMaxC / 32; ++k) { const int c = lane + 32 * k; q[k] = c < C ? qd[i * C + c] : 0.0; }
+  const int64_t b = cand_begin[i], e = cand_end[i];
+  int64_t arg = -1;
+  double dm = INFINITY;
+  for (int64_t r = b; r < e; ++r) {
+    const double* row = cand + r * C;
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < kNCMaxC / 32; ++k) {
+      const int c = lane + 32 * k;
+      if (c < C) { const double t = row[c] - q[k]; s += t * t; }
+    }
+    s = warp_sum(s);
+    if (s < dm || (s != s && dm == dm)) { dm = s; arg = r; }   // numpy's argmin: the first NaN wins
+  }
+  if (lane == 0) { best[i] = arg; if (d_min) d_min[i] = dm; }
 }
 
 template <typename T>
@@ -328,5 +364,89 @@ extern "C" int pxr_obs_descriptors(pxr_ctx* ctx, const pxr_ba_desc* desc, const 
   PXR_TRY(launch_fm_eval(ctx, b.dtype, b.C, 0, b.interp.use_float_simd != 0, a, &np));
   PXR_CUDA(cudaMemcpyAsync(out_desc, dsc.p, (size_t)b.n_obs * b.C * 8, cudaMemcpyDeviceToHost, ctx->stream));
   PXR_CUDA(cudaStreamSynchronize(ctx->stream));
+  return PXR_OK;
+}
+
+extern "C" int pxr_query_match_run(pxr_ctx* ctx, int32_t n_queries, const void* const* patch_blocks,
+                                   const int64_t* patch_counts, const int32_t* corner, const double* scale, double ups,
+                                   int32_t ph, int32_t pw, int32_t channels, int32_t patch_dtype, int64_t n_items,
+                                   const int32_t* item_query, const int64_t* item_patch, const double* xy,
+                                   const int64_t* cand_begin, const int64_t* cand_end, const double* cand, int64_t n_cand,
+                                   int32_t cand_on_device,
+                                   const pxr_interp_config* interp, int64_t* best, double* d_min, double* out_desc) {
+  // ---- arguments, before the context
+  if (n_queries < 0 || n_items < 0 || n_cand < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "negative count");
+  if ((n_queries > 0 && (!patch_blocks || !patch_counts)) ||
+      (n_items > 0 && (!item_query || !item_patch || !xy || !cand_begin || !cand_end || !best)) || (n_cand > 0 && !cand))
+    return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  if (interp && interp->check_bounds) return fail(PXR_ERR_UNSUPPORTED, "check_bounds=true is not supported on this path");
+  if (!fm_supported(patch_dtype, channels) || channels > kNCMaxC)
+    return fail(PXR_ERR_UNSUPPORTED, "Unsupported dimensions (CHANNELS=%d, dtype=%d, N_NODES=1).", channels, patch_dtype);
+  if (ph < 1 || pw < 1) return fail(PXR_ERR_INVALID_ARGUMENT, "bad patch size");
+  if (!(ups > 0.0)) return fail(PXR_ERR_INVALID_ARGUMENT, "upsampling_factor must be > 0");
+  std::vector<int64_t> first((size_t)n_queries + 1, 0);
+  for (int q = 0; q < n_queries; ++q) {
+    if (patch_counts[q] < 0) return fail(PXR_ERR_INVALID_ARGUMENT, "patch_counts[%d] < 0", q);
+    if (patch_counts[q] > 0 && !patch_blocks[q]) return fail(PXR_ERR_INVALID_ARGUMENT, "patch block %d is NULL", q);
+    first[q + 1] = first[q] + patch_counts[q];
+  }
+  if (first[n_queries] > 0 && (!corner || !scale)) return fail(PXR_ERR_INVALID_ARGUMENT, "a required array is NULL");
+  // patch pixel coordinates, FeaturePatch::ToPixelCoordinates, as pxr_interpolate_descriptors computes them
+  std::vector<double> uv((size_t)n_items * 2);
+  std::vector<int64_t> gpatch((size_t)n_items);
+  for (int64_t i = 0; i < n_items; ++i) {
+    const int q = item_query[i];
+    if (q < 0 || q >= n_queries) return fail(PXR_ERR_INVALID_ARGUMENT, "item_query[%lld] out of range", (long long)i);
+    if (item_patch[i] < 0 || item_patch[i] >= patch_counts[q])
+      return fail(PXR_ERR_INVALID_ARGUMENT, "item_patch[%lld] is not a patch of query %d", (long long)i, q);
+    if (cand_begin[i] < 0 || cand_end[i] < cand_begin[i] || cand_end[i] > n_cand)
+      return fail(PXR_ERR_INVALID_ARGUMENT, "candidate range of item %lld is out of bounds", (long long)i);
+    const int64_t pi = first[q] + item_patch[i];
+    gpatch[i] = pi;
+    uv[2 * i] = (xy[2 * i] * scale[2 * pi] - 0.5 - (double)corner[2 * pi]) * ups;
+    uv[2 * i + 1] = (xy[2 * i + 1] * scale[2 * pi + 1] - 0.5 - (double)corner[2 * pi + 1]) * ups;
+  }
+  PXR_TRY(require_ctx(ctx));
+  pxr_interp_config ic; if (interp) ic = *interp; else pxr_default_interp_config(&ic);
+  if (n_items == 0) return PXR_OK;
+  PXR_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t s = ctx->stream;
+  // the query blocks back to back in one slab (device blocks are copied on the device)
+  const size_t per = (size_t)ph * pw * channels * dtype_bytes(patch_dtype);
+  std::vector<const void*> srcs((size_t)n_queries);
+  std::vector<size_t> sizes((size_t)n_queries);
+  static const uint8_t kNoPatch = 0;
+  for (int q = 0; q < n_queries; ++q) {
+    srcs[q] = patch_counts[q] > 0 ? patch_blocks[q] : &kNoPatch;
+    sizes[q] = (size_t)patch_counts[q] * per;
+  }
+  DevBuf<uint8_t> dp; DevBuf<double> duv, ddesc, dcand, dmin; DevBuf<int64_t> dip, dcb, dce, dbest;
+  PXR_TRY(dp.alloc(std::max<size_t>((size_t)first[n_queries] * per, 16)));
+  PXR_TRY(upload_segments(ctx, dp.p, srcs.data(), sizes.data(), n_queries, nullptr, s));
+  PXR_TRY(duv.upload(uv.data(), uv.size(), s));
+  PXR_TRY(dip.upload(gpatch.data(), gpatch.size(), s));
+  PXR_TRY(dcb.upload(cand_begin, (size_t)n_items, s));
+  PXR_TRY(dce.upload(cand_end, (size_t)n_items, s));
+  const double* cp = cand;
+  if (!cand_on_device && n_cand > 0) { PXR_TRY(dcand.upload(cand, (size_t)n_cand * channels, s)); cp = dcand.p; }
+  PXR_TRY(ddesc.alloc((size_t)n_items * channels));
+  PXR_TRY(dbest.alloc((size_t)n_items));
+  PXR_TRY(dmin.alloc((size_t)n_items));
+  // the query descriptors: K1 in descriptor mode, as pxr_interpolate_descriptors runs it
+  FmEvalArgs a;
+  a.uv = duv.p; a.item_patch = dip.p; a.item_ref = nullptr;
+  a.patches = dp.p; a.ph = ph; a.pw = pw; a.refs = nullptr;
+  a.begin = 0; a.end = n_items; a.item_index = nullptr; a.out = nullptr; a.residuals = nullptr; a.desc = ddesc.p;
+  a.loss.type = 0; a.loss.a = 1.0;
+  a.l2_normalize = ic.l2_normalize;
+  int np = 0;
+  PXR_TRY(launch_fm_eval(ctx, patch_dtype, channels, 0, ic.use_float_simd != 0, a, &np));
+  PXR_LAUNCH(ctx, nearest_candidate_kernel, (unsigned)cdiv(n_items * 32, 256), 256, 0, ddesc.p, dcb.p, dce.p, cp, n_items,
+             (int)channels, dbest.p, dmin.p);
+  PXR_CUDA(cudaGetLastError());
+  PXR_CUDA(cudaMemcpyAsync(best, dbest.p, (size_t)n_items * 8, cudaMemcpyDeviceToHost, s));
+  if (d_min) PXR_CUDA(cudaMemcpyAsync(d_min, dmin.p, (size_t)n_items * 8, cudaMemcpyDeviceToHost, s));
+  if (out_desc) PXR_CUDA(cudaMemcpyAsync(out_desc, ddesc.p, (size_t)n_items * channels * 8, cudaMemcpyDeviceToHost, s));
+  PXR_CUDA(cudaStreamSynchronize(s));
   return PXR_OK;
 }

@@ -153,6 +153,41 @@ class QBAResult(C.Structure):          # pxr_qba_result
                 ("block_evaluations", C.c_int64)]
 
 
+def _patch_blocks(blocks):
+    """one patch block per query, host numpy or device memory (anything with `.ptr` or __cuda_array_interface__) ->
+    (ctypes pointer array, patch counts, (ph, pw, channels), dtype id)"""
+    ptrs, counts, shape, dtype = [], [], None, None
+    for b in blocks:
+        cai = getattr(b, "__cuda_array_interface__", None)
+        if getattr(b, "ptr", None) is not None:
+            p, shp, dt = int(b.ptr), tuple(b.shape), np.dtype(b.dtype)
+        elif cai is not None:
+            p, shp, dt = int(cai["data"][0]), tuple(cai["shape"]), np.dtype(cai["typestr"])
+        else:
+            if b.dtype not in DTYPE_IDS or not b.flags["C_CONTIGUOUS"] or b.ndim != 4:
+                raise ValueError("patch blocks must be C-contiguous [N,H,W,C] f16/f32/f64 arrays")
+            p, shp, dt = b.ctypes.data, tuple(b.shape), np.dtype(b.dtype)
+        if shape is not None and (shp[1:] != shape or dt != dtype):
+            raise ValueError("patch blocks must share one dtype and patch shape")
+        shape, dtype = shp[1:], dt
+        ptrs.append(p); counts.append(shp[0])
+    return ((C.c_void_p * max(len(ptrs), 1))(*ptrs), np.array(counts, np.int64), shape if shape is not None else (1, 1, 8),
+            DTYPE_IDS[dtype] if dtype is not None else 0)
+
+
+class QKADesc(C.Structure):            # pxr_qka_desc
+    _fields_ = [("n_queries", C.c_int32), ("kp_begin", C.c_void_p), ("patch_blocks", C.c_void_p),
+                ("patch_counts", C.c_void_p), ("patches_are_sparse", C.c_void_p), ("keypoints", C.c_void_p),
+                ("kp_patch", C.c_void_p), ("desc_begin", C.c_void_p), ("descs", C.c_void_p), ("corner", C.c_void_p),
+                ("scale", C.c_void_p), ("upsampling_factor", C.c_double), ("bound", C.c_double), ("ph", C.c_int32),
+                ("pw", C.c_int32), ("channels", C.c_int32), ("patch_dtype", C.c_int32), ("max_wave_bytes", C.c_double)]
+
+
+class QKAResult(C.Structure):          # pxr_qka_result
+    _fields_ = [("status", C.c_int32), ("num_residual_blocks", C.c_int32), ("initial_cost", C.c_double),
+                ("final_cost", C.c_double), ("num_successful_steps", C.c_int32), ("num_unsuccessful_steps", C.c_int32),
+                ("num_iterations", C.c_int32), ("termination_type", C.c_int32)]
+
 class QBABatch:
     """numpy arrays of a batch of query bundle adjustments + the ctypes view (pxr_qba_desc).  Per query: camera model,
     params [12] (in/out), constancy mask, qvec / tvec (in/out), a patch block [n_q, H, W, C] (host numpy array or
@@ -179,25 +214,7 @@ class QBABatch:
         if len(patch_blocks) != nq:
             raise ValueError("one patch block per query")
         self.patch_blocks = list(patch_blocks)
-        ptrs, counts, shape, dtype = [], [], None, None
-        for b in self.patch_blocks:
-            cai = getattr(b, "__cuda_array_interface__", None)
-            if getattr(b, "ptr", None) is not None:
-                p, shp, dt = int(b.ptr), tuple(b.shape), np.dtype(b.dtype)
-            elif cai is not None:
-                p, shp, dt = int(cai["data"][0]), tuple(cai["shape"]), np.dtype(cai["typestr"])
-            else:
-                if b.dtype not in DTYPE_IDS or not b.flags["C_CONTIGUOUS"] or b.ndim != 4:
-                    raise ValueError("patch blocks must be C-contiguous [N,H,W,C] f16/f32/f64 arrays")
-                p, shp, dt = b.ctypes.data, tuple(b.shape), np.dtype(b.dtype)
-            if shape is not None and (shp[1:] != shape or dt != dtype):
-                raise ValueError("patch blocks must share one dtype and patch shape")
-            shape, dtype = shp[1:], dt
-            ptrs.append(p); counts.append(shp[0])
-        self._ptrs = (C.c_void_p * max(nq, 1))(*ptrs)
-        self.patch_counts = np.array(counts, np.int64)
-        self.ph, self.pw, self.channels = shape if shape is not None else (1, 1, 8)
-        self.patch_dtype = DTYPE_IDS[dtype] if dtype is not None else 0
+        self._ptrs, self.patch_counts, (self.ph, self.pw, self.channels), self.patch_dtype = _patch_blocks(self.patch_blocks)
         self.corner = _as(corner, np.int32, (-1, 2))
         self.scale = _as(scale, np.float64, (-1, 2))
         self.upsampling_factor = float(upsampling_factor)
@@ -663,3 +680,94 @@ class KAProblem:
     def merge_shard(self, sub, kp_global):
         """write a solved shard's keypoints back"""
         self.keypoints[kp_global] = sub.keypoints
+
+
+class QKABatch(KAProblem):
+    """numpy arrays of a batch of query keypoint adjustments + the ctypes view (pxr_qka_desc).  Per query: a keypoint
+    range kp_begin, a patch block [n_q, H, W, C] (host numpy array or device memory) with its corners and scales, and
+    whether its map is sparse; per keypoint: its patch within the query's block and a range of fixed fp64 descriptors,
+    one residual block each.  It is also the KAProblem of the same problems (query mode, one problem per query, the
+    blocks back to back) when the blocks are host arrays: desc() gives that pxr_ka_desc, qka_desc() the batched one.
+    `results` holds one dict per query (the pxr_qka_result fields) once solved."""
+
+    def __init__(self, keypoints, kp_begin, kp_patch, desc_begin, descs, patch_blocks, corner, scale, patches_are_sparse,
+                 bound=4.0, upsampling_factor=1.0, max_wave_bytes=0.0):
+        self.keypoints = _as(keypoints, np.float64, (-1, 2)).copy()
+        self.kp_begin = _as(kp_begin, np.int64)
+        self.kp_patch_local = _as(kp_patch, np.int64)
+        self.desc_begin = _as(desc_begin, np.int64)
+        nq, nk = len(self.kp_begin) - 1, len(self.keypoints)
+        self.patch_blocks = list(patch_blocks)
+        if len(self.patch_blocks) != nq:
+            raise ValueError("one patch block per query")
+        self._qptrs, self.patch_counts, shape, self.patch_dtype = _patch_blocks(self.patch_blocks)
+        self.ph, self.pw, ch = shape
+        self.ref_desc = np.ascontiguousarray(descs, np.float64).reshape(-1, ch) if len(descs) else np.zeros((0, ch))
+        self.corner = _as(corner, np.int32, (-1, 2))
+        self.scale = _as(scale, np.float64, (-1, 2))
+        self.sparse = _as(patches_are_sparse, np.uint8)
+        self.bound = float(bound)
+        self.upsampling_factor = float(upsampling_factor)
+        self.max_wave_bytes = float(max_wave_bytes)
+        self._shape = (int(self.patch_counts.sum()), self.ph, self.pw, ch)
+        self._dtype = {v: k for k, v in DTYPE_IDS.items()}[self.patch_dtype]
+        # the same problems as one pxr_ka_desc: edge = (keypoint, descriptor), problem = query
+        counts = np.diff(self.desc_begin) if nk else np.zeros(0, np.int64)
+        self.edge_src = np.repeat(np.arange(nk, dtype=np.int64), counts)
+        self.edge_dst = np.arange(len(self.edge_src), dtype=np.int64)
+        self.edge_problem = np.repeat(np.arange(nq, dtype=np.int32), np.diff(self.desc_begin[self.kp_begin])) if nk else \
+            np.zeros(0, np.int32)
+        self.edge_weight = None
+        self.kp_const = np.zeros(nk, np.uint8)
+        self.n_problems = nq
+        first = np.concatenate([[0], np.cumsum(self.patch_counts)])[:-1] if nq else np.zeros(0, np.int64)
+        self.kp_patch = self.kp_patch_local + np.repeat(first, np.diff(self.kp_begin)).astype(np.int64)
+        self.patches = None
+        self.results = [dict(status=PXR_OK, num_residual_blocks=int(self.desc_begin[self.kp_begin[q + 1]] -
+                                                                    self.desc_begin[self.kp_begin[q]]) if nk else 0,
+                             initial_cost=0.0, final_cost=0.0, num_successful_steps=0, num_unsuccessful_steps=0,
+                             num_iterations=0, termination_type=1) for q in range(nq)]
+
+    @property
+    def n_queries(self):
+        return len(self.kp_begin) - 1
+
+    @property
+    def patches_are_sparse(self):
+        """the one flag of the pxr_ka_desc view: it exists when the queries agree or when bound > 0 decides alone"""
+        if self.bound <= 0 and len(set(self.sparse.tolist())) > 1:
+            raise ValueError("the queries mix sparse and dense maps with bound <= 0: no single pxr_ka_desc holds them")
+        return bool(self.sparse[0]) if len(self.sparse) else True
+
+    def desc(self):
+        if any(not isinstance(b, np.ndarray) for b in self.patch_blocks):
+            raise ValueError("the pxr_ka_desc view of a query batch takes host patch blocks")
+        d = KADesc()
+        d.n_keypoints = len(self.keypoints)
+        d.keypoints = _ptr(self.keypoints); d.kp_const = _ptr(self.kp_const); d.kp_patch = _ptr(self.kp_patch)
+        d.n_edges = len(self.edge_src)
+        d.edge_src = _ptr(self.edge_src); d.edge_dst = _ptr(self.edge_dst); d.edge_problem = _ptr(self.edge_problem)
+        d.n_problems = self.n_problems
+        d.n_patches = self._shape[0]
+        d.n_patch_blocks = self.n_queries
+        d.patch_block_ptrs = C.cast(self._qptrs, C.c_void_p); d.patch_block_counts = _ptr(self.patch_counts)
+        d.patch_dtype = self.patch_dtype
+        d.ph, d.pw, d.channels = self._shape[1:]
+        d.corner = _ptr(self.corner); d.scale = _ptr(self.scale)
+        d.upsampling_factor = self.upsampling_factor
+        d.bound = self.bound
+        d.patches_are_sparse = int(self.patches_are_sparse)
+        d.ref_desc = _ptr(self.ref_desc); d.n_ref_desc = len(self.ref_desc)
+        return d
+
+    def qka_desc(self):
+        d = QKADesc()
+        d.n_queries = self.n_queries
+        d.kp_begin = _ptr(self.kp_begin); d.patch_blocks = C.cast(self._qptrs, C.c_void_p)
+        d.patch_counts = _ptr(self.patch_counts); d.patches_are_sparse = _ptr(self.sparse)
+        d.keypoints = _ptr(self.keypoints); d.kp_patch = _ptr(self.kp_patch_local); d.desc_begin = _ptr(self.desc_begin)
+        d.descs = _ptr(self.ref_desc); d.corner = _ptr(self.corner); d.scale = _ptr(self.scale)
+        d.upsampling_factor = self.upsampling_factor; d.bound = self.bound
+        d.ph, d.pw, d.channels, d.patch_dtype = self.ph, self.pw, self._shape[3], self.patch_dtype
+        d.max_wave_bytes = self.max_wave_bytes
+        return d

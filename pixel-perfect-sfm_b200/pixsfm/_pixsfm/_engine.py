@@ -368,12 +368,24 @@ def memcpy_d2h(host_array, dev_ptr, nbytes, ctx=None):
 
 
 def ka_run(problem, interp=None, options=None, ctx=None):
-    """pxr_ka_run == FeatureMetricKeypointOptimizer.run: refines problem.keypoints IN PLACE."""
+    """pxr_ka_run == FeatureMetricKeypointOptimizer.run: refines problem.keypoints IN PLACE.  A _capi.QKABatch (one
+    query-mode problem per query) is solved by pxr_qka_run, which also fills problem.results per query and adds
+    `n_waves` to the summary."""
     ctx = ctx or _capi.default_context()
     interp = interp or _capi.default_interp()
     options = options or _capi.default_ka_options()
-    d = problem.desc()
     s = _capi.make_summary(0)
+    if isinstance(problem, _capi.QKABatch):
+        d = problem.qka_desc()
+        res = (_capi.QKAResult * max(problem.n_queries, 1))()
+        nw = C.c_int32()
+        _capi.check(ctx.lib.pxr_qka_run(ctx.handle, C.byref(d), C.byref(interp), C.byref(options), res, C.byref(nw),
+                                        C.byref(s)))
+        problem.results = [{f[0]: getattr(res[q], f[0]) for f in _capi.QKAResult._fields_} for q in range(problem.n_queries)]
+        out = _capi.summary_to_dict(s)
+        out["n_waves"] = nw.value
+        return out
+    d = problem.desc()
     _capi.check(ctx.lib.pxr_ka_run(ctx.handle, C.byref(d), C.byref(interp), C.byref(options), C.byref(s)))
     return _capi.summary_to_dict(s)
 
@@ -491,3 +503,50 @@ def interpolate_patches(patches, corners, scales, item_patch, xys, interp=None, 
         int(patches.shape[2]), int(patches.shape[3]), _p(corners), _p(scales), C.c_double(upsampling_factor),
         C.c_int64(len(xys)), _p(item_patch), _p(xys), C.byref(interp), _p(out)))
     return out
+
+
+def query_match_run(blocks, corners, scales, item_query, item_patch, xys, cand_begin, cand_end, cand, interp=None,
+                    with_desc=False, ctx=None):
+    """pxr_query_match_run: per item the descriptor of patch item_patch[i] of query item_query[i]'s block (host numpy
+    or device memory) at xys[i], and the first of the candidate rows [cand_begin[i], cand_end[i]) of `cand` (a host
+    [n, C] float64 array, or device memory with __cuda_array_interface__, read in place) closest to it.
+    -> (best row [n_items] int64, -1 for an empty range; squared distance [n_items]; descriptors [n_items, C] or None)"""
+    interp = interp or _capi.default_interp()
+    ptrs, counts, (ph, pw, ch), dt = _capi._patch_blocks(blocks)
+    corners = np.ascontiguousarray(corners, np.int32).reshape(-1, 2)
+    scales = np.ascontiguousarray(scales, np.float64).reshape(-1, 2)
+    item_query = np.ascontiguousarray(item_query, np.int32)
+    item_patch = np.ascontiguousarray(item_patch, np.int64)
+    xys = np.ascontiguousarray(xys, np.float64).reshape(-1, 2)
+    cb = np.ascontiguousarray(cand_begin, np.int64); ce = np.ascontiguousarray(cand_end, np.int64)
+    n = len(item_query)
+    if not (len(item_patch) == len(xys) == len(cb) == len(ce) == n):
+        raise ValueError("one query, patch, point and candidate range per item")
+    cai = getattr(cand, "__cuda_array_interface__", None)
+    if cai is not None:
+        shape = tuple(cai["shape"])
+        contiguous = cai.get("strides") is None or tuple(cai["strides"]) == (ch * 8, 8)
+        if np.dtype(cai["typestr"]) != np.dtype("<f8") or len(shape) != 2 or (shape[0] and shape[1] != ch) or not contiguous:
+            raise ValueError("the candidate table must be a C-contiguous [n, %d] float64 array" % ch)
+        n_cand, cptr, on_dev = int(shape[0]), C.c_void_p(int(cai["data"][0])), 1
+    else:
+        cand = np.ascontiguousarray(cand, np.float64)
+        if len(cand) and (cand.ndim != 2 or cand.shape[1] != ch):
+            raise ValueError("the candidate table must be [n, %d] (one descriptor of the patches' channels per row)" % ch)
+        cand = cand.reshape(-1, ch)
+        n_cand, cptr, on_dev = len(cand), _p(cand), 0
+    ctx = ctx or _capi.default_context()
+    best, dmin = np.zeros(n, np.int64), np.zeros(n)
+    desc = np.zeros((n, ch)) if with_desc else None
+    _capi.check(ctx.lib.pxr_query_match_run(
+        ctx.handle, C.c_int32(len(counts)), C.cast(ptrs, C.c_void_p), _p(counts), _p(corners), _p(scales), C.c_double(1.0),
+        int(ph), int(pw), int(ch), int(dt), C.c_int64(n), _p(item_query), _p(item_patch), _p(xys), _p(cb), _p(ce), cptr,
+        C.c_int64(n_cand), int(on_dev), C.byref(interp), _p(best), _p(dmin), _p(desc)))
+    return best, dmin, desc
+
+
+def device_array(a):
+    """a host array copied to device memory (a torch CUDA tensor: its __cuda_array_interface__ is what the library
+    reads; freed with the tensor)"""
+    import torch
+    return torch.as_tensor(np.ascontiguousarray(a), device="cuda")

@@ -88,6 +88,103 @@ def find_nearest_references(query_fmap, references, keypoints, point3D_ids, inte
     return out
 
 
+_MISSING_OBS = "Missing observations in references. Extract references with option keep_observations=True."
+
+
+def observation_table(references, point_ids):
+    """the stored observation descriptors of the given 3D points back to back: (rows [n, C] float64, {point id: (first
+    row, number of rows)}).  Raises find_nearest_references' error for a point without observations."""
+    rows, where, n = [], {}, 0
+    for pid in point_ids:
+        if pid in where:
+            continue
+        obs = getattr(references[pid], "observations", None)
+        if not obs:
+            raise ValueError(_MISSING_OBS)
+        where[pid] = (n, len(obs))
+        n += len(obs)
+        rows.extend(np.asarray(o, np.float64).reshape(-1) for o in obs)
+    return (np.array(rows) if rows else np.zeros((0, 0))), where
+
+
+def find_nearest_references_batch(items, interpolation_config, _table=None):
+    """find_nearest_references for many queries in one pxr_query_match_run.  items: (query_fmap, references, keypoints,
+    point3D_ids[, patch_idxs]) -> per query the list find_nearest_references returns.  The candidates of a
+    correspondence are its 3D point's stored observations; `_table` = (rows, {point id: (first row, count)}) passes a
+    table already packed (rows may be device memory) instead of packing the references again."""
+    interp = interpolation_config if isinstance(interpolation_config, InterpolationConfig) else InterpolationConfig(interpolation_config or {})
+    interp.validate_for_device()
+    items = list(items)
+    blocks, corners, scales, iq, ip, xys, pids = [], [], [], [], [], [], []
+    for k, it in enumerate(items):
+        fmap, references, keypoints, point3D_ids = it[:4]
+        patch_idxs = it[4] if len(it) > 4 else None
+        keypoints = np.asarray(keypoints, np.float64).reshape(-1, 2)
+        idxs = list(range(len(keypoints))) if patch_idxs is None else list(patch_idxs)
+        for pid in point3D_ids:
+            if (pid not in _table[1]) if _table is not None else not getattr(references[pid], "observations", None):
+                raise ValueError("query %d: %s" % (k, _MISSING_OBS))
+        blocks.append(fmap.patches)
+        corners.append(np.asarray(fmap.corners, np.int32).reshape(-1, 2))
+        scales.append(np.tile(fmap.scale, (fmap.size(), 1)))
+        for i, pid in enumerate(point3D_ids):
+            iq.append(k); ip.append(fmap.local_index(idxs[i])); xys.append(keypoints[i]); pids.append(pid)
+    if _table is None:
+        refs_of = {}
+        for k, it in enumerate(items):
+            for pid in it[3]:
+                refs_of.setdefault(pid, it[1][pid])
+        rows, where = observation_table(refs_of, list(refs_of)) if refs_of else (np.zeros((0, 0)), {})
+        rows = np.asarray(rows, np.float64)
+    else:
+        rows, where = _table
+    cb = np.array([where[p][0] for p in pids], np.int64)
+    ce = np.array([where[p][0] + where[p][1] for p in pids], np.int64)
+    out = [[] for _ in items]
+    if not pids:
+        return out
+    ic = _capi.default_interp(interp.l2_normalize, interp.use_float_simd)
+    best, _, _ = _engine.query_match_run(blocks, np.concatenate(corners), np.concatenate(scales), iq, ip, xys, cb, ce, rows, ic)
+    for k, pid, b, first in zip(iq, pids, best, cb):
+        if b < 0:          # an empty candidate range: the point has no stored observations
+            raise ValueError("query %d: %s" % (k, _MISSING_OBS))
+        obs = items[k][1][pid].observations
+        out[k].append(np.asarray(obs[int(b - first)], np.float64).reshape(1, -1).copy())
+    return out
+
+
+def feature_inliers_batch(items, interpolation_config, thresh):
+    """find_feature_inliers (localization/main.py) for many queries in one pxr_query_match_run.  items: (points2D, fmap,
+    references, point2D_idxs or None) -> per query one bool per correspondence: a correspondence whose reference is one
+    ndarray is an inlier when the interpolated descriptor lies within `thresh` (L2) of it; others always are"""
+    items = list(items)
+    if thresh < 0.0:
+        return [[True] * len(it[0]) for it in items]
+    interp = interpolation_config if isinstance(interpolation_config, InterpolationConfig) else InterpolationConfig(interpolation_config or {})
+    interp.validate_for_device()
+    blocks, corners, scales, iq, ip, xys, cand, cb, ce, tested = [], [], [], [], [], [], [], [], [], []
+    for k, (p2Ds, fmap, references, idxs) in enumerate(items):
+        idxs = list(range(len(p2Ds)) if idxs is None else idxs)
+        blocks.append(fmap.patches)
+        corners.append(np.asarray(fmap.corners, np.int32).reshape(-1, 2))
+        scales.append(np.tile(fmap.scale, (fmap.size(), 1)))
+        for i, (xy, ref) in enumerate(zip(np.asarray(p2Ds, np.float64).reshape(-1, 2), references)):
+            if not isinstance(ref, np.ndarray):
+                continue
+            iq.append(k); ip.append(fmap.local_index(idxs[i]))
+            xys.append(xy); cb.append(len(cand)); ce.append(len(cand) + 1); cand.append(np.asarray(ref, np.float64).reshape(-1))
+            tested.append((k, i))
+    out = [[True] * len(it[0]) for it in items]
+    if not tested:
+        return out
+    ic = _capi.default_interp(interp.l2_normalize, interp.use_float_simd)
+    _, dmin, _ = _engine.query_match_run(blocks, np.concatenate(corners), np.concatenate(scales), iq, ip, xys, cb, ce,
+                                         np.array(cand), ic)
+    for (k, i), d in zip(tested, dmin):
+        out[k][i] = bool(np.sqrt(d) <= thresh)
+    return out
+
+
 class QueryKeypointOptimizer:
     """_localization.QueryKeypointOptimizer(options, interpolation).run(keypoints, fmap, references, patch_idxs=None,
     inliers=None) -> bool; `keypoints` ([N,2] float64) is refined IN PLACE."""
@@ -148,6 +245,94 @@ class QueryKeypointOptimizer:
 
     def summary(self):
         return self._summary
+
+    # ---- batched: many queries in one pxr_qka_run
+    def pack_batch(self, queries, max_wave_bytes=0.0):
+        """the problems build_problem makes for every query of `queries` (argument tuples as run takes them:
+        (keypoints, fmap, references[, patch_idxs[, inliers]])) as one _capi.QKABatch, and per query the indices of
+        the keypoints it holds.  Feature maps may hold host (numpy) or device patches (DevicePatches)."""
+        self.interp.validate_for_device()
+        kps, kp_begin, kp_patch, desc_begin, descs, blocks, corners, scales, sparse, used_of = ([] for _ in range(10))
+        kp_begin.append(0); desc_begin.append(0)
+        channels = dtype = None
+        for k, args in enumerate(queries):
+            keypoints, fmap, references = args[:3]
+            patch_idxs = args[3] if len(args) > 3 else None
+            inliers = args[4] if len(args) > 4 else None
+            try:
+                if not isinstance(keypoints, np.ndarray) or keypoints.dtype != np.float64 or keypoints.ndim != 2 or \
+                        keypoints.shape[1] != 2:
+                    raise ValueError("keypoints must be a [N,2] float64 array")
+                n = len(keypoints)
+                if len(references) != n:
+                    raise ValueError("references.size() != keypoints.rows()")
+                if patch_idxs is not None and len(patch_idxs) != n:
+                    raise ValueError("patch_idxs.size() != keypoints.rows()")
+                if len(self.interp.nodes) != 1 or fmap.channels not in (8, 16, 32, 64, 128):
+                    raise ValueError("Unsupported dimensions (CHANNELS,N_NODES).")
+                if channels is not None and fmap.channels != channels:
+                    raise ValueError("every query of a batch must have the same channel count")
+                dt = np.dtype(getattr(fmap.patches, "dtype"))
+                if dtype is not None and dt != dtype:
+                    raise ValueError("every query of a batch must have the same patch dtype")
+            except ValueError as e:
+                raise ValueError("query %d: %s" % (k, e)) from None
+            channels, dtype = fmap.channels, dt
+            used = []
+            for i in range(n):
+                if inliers is not None and not inliers[i]:
+                    continue
+                ds = _descriptors_of(references[i], fmap.channels)
+                if not ds:
+                    continue
+                used.append(i)
+                kps.append(keypoints[i]); kp_patch.append(fmap.local_index(i if patch_idxs is None else patch_idxs[i]))
+                descs.extend(ds); desc_begin.append(len(descs))
+            used_of.append(used)
+            kp_begin.append(len(kps))
+            blocks.append(fmap.patches)
+            corners.append(np.asarray(fmap.corners, np.int32).reshape(-1, 2))
+            scales.append(np.tile(fmap.scale, (fmap.size(), 1)))
+            sparse.append(bool(fmap.is_sparse))
+        batch = _capi.QKABatch(np.array(kps).reshape(-1, 2), kp_begin, kp_patch, desc_begin,
+                               np.array(descs) if descs else np.zeros((0, channels or 8)), blocks,
+                               np.concatenate(corners) if corners else np.zeros((0, 2), np.int32),
+                               np.concatenate(scales) if scales else np.zeros((0, 2)), sparse,
+                               bound=float(self.options.bound), max_wave_bytes=max_wave_bytes)
+        return batch, used_of
+
+    def run_batch(self, queries, max_wave_bytes=0.0):
+        """run() for every query of `queries` (argument tuples (keypoints, fmap, references[, patch_idxs[, inliers]]))
+        in one pxr_qka_run: each query's keypoints are refined IN PLACE.  -> one bool per query, what run() returns
+        (False: no residual block).  summaries() gives each query's summary; its total_time_s is that of the whole
+        batch.  A query whose initial cost is not finite gets what run() gives it: its keypoints as the solver leaves
+        them, True, and a summary with that cost (a warning names the query)."""
+        queries = list(queries)
+        batch, used_of = self.pack_batch(queries, max_wave_bytes)
+        so = self.solver_options()
+        ic = _capi.default_interp(self.interp.l2_normalize, self.interp.use_float_simd)
+        tot = _engine.ka_run(batch, ic, so)
+        ch = batch.channels
+        self._summaries, ok = [], []
+        for k, (args, r, used) in enumerate(zip(queries, batch.results, used_of)):
+            if r["num_residual_blocks"] == 0:
+                self._summaries.append(None); ok.append(False)
+                continue
+            if r["status"] != _capi.PXR_OK:
+                logger.warning("QKA query %d: initial cost is not finite", k)
+            kb, ke = int(batch.kp_begin[k]), int(batch.kp_begin[k + 1])
+            args[0][used] = batch.keypoints[kb:ke]
+            nres = max(1, r["num_residual_blocks"] * ch)
+            s = dict(r, num_residuals=r["num_residual_blocks"] * ch, num_inner_iteration_steps=0,
+                     total_time_s=tot["total_time_s"], solve_time_s=tot["solve_time_s"], iterations=[])
+            self._summaries.append(_Summary(s, num_residuals_reduced=nres))
+            ok.append(True)
+        logger.info("QKA Time: %.4gs for %d queries", tot["total_time_s"], len(queries))
+        return ok
+
+    def summaries(self):
+        """per-query summaries of the last run_batch (None for a query that was not solved)"""
+        return getattr(self, "_summaries", [])
 
 
 class QueryBundleOptimizer:

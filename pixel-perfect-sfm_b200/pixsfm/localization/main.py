@@ -4,12 +4,17 @@ calls pycolmap.absolute_pose_estimation, which is not part of this package)."""
 import numpy as np
 
 from .. import defaults
-from .._pixsfm import _localization as loc
+from .._pixsfm import _engine, _localization as loc
 from ..util.conf import merge, to_ctr
 from ..util.refine import level_order, optimizer_options
 
 resolve_level_indices = level_order          # the reference's name (util/misc.py:19-23)
 to_optim_ctr = optimizer_options             # the reference's name (util/misc.py:30-36)
+
+
+def st_needs_features(states):
+    """the queries' states need reference descriptors (QKA or QBA runs)"""
+    return bool(states) and states[0]["require_feats"]
 
 
 def find_feature_inliers(p2Ds, fmap, references, interpolation_config, thresh=-1, point2D_idxs=None):
@@ -73,8 +78,40 @@ class QueryKeypointAdjuster:
         for level in level_order(self.conf.level_indices, len(query_fmaps)):
             self.refine(pnp_points2D, query_fmaps[level], references[level], point2D_idxs=point2D_idxs)
 
-    def refine_stacked(self, pnp_points2D, fmap, references, point2D_idxs, inliers=None):
-        """correspondences that share a keypoint are stacked into ONE keypoint with several targets"""
+    def refine_batch(self, queries, max_wave_bytes=0.0):
+        """refine() for every query of `queries`, tuples (pnp_points2D, fmap, references[, point2D_idxs]): the feature
+        inlier test of all queries in one pxr_query_match_run, then one batched solve (QueryKeypointOptimizer.run_batch)"""
+        queries = [tuple(q) + (None,) * (4 - len(q)) for q in queries]
+        inl = loc.feature_inliers_batch(queries, to_ctr(self.conf.interpolation), self.conf.feature_inlier_thresh)
+        items, stacked = [], []
+        for (p2D, fmap, refs, idxs), inliers in zip(queries, inl):
+            if self.conf.stack_correspondences:
+                kps, targets, slots, admitted, where = self._stack(p2D, refs, idxs, inliers)
+                items.append((kps, fmap, targets, slots, admitted)); stacked.append((p2D, kps, where))
+            else:
+                items.append((p2D, fmap, refs, idxs, inliers))
+        self.solver = loc.QueryKeypointOptimizer(self.solver.options, self.solver.interp)
+        self.solver.run_batch(items, max_wave_bytes)
+        for p2D, kps, where in stacked:
+            for k, slot in enumerate(where):
+                p2D[k] = kps[slot]
+
+    def refine_multilevel_batch(self, queries, max_wave_bytes=0.0):
+        """refine_multilevel() for every query of `queries`, tuples (pnp_points2D, query_fmaps, references[,
+        point2D_idxs]) with one fmap and one reference list per level: one batched refine per level"""
+        queries = list(queries)
+        if not queries:
+            return
+        n_levels = len(queries[0][1])
+        if any(len(q[1]) != n_levels for q in queries):
+            raise ValueError("every query of a batch must have the same number of feature levels")
+        for level in level_order(self.conf.level_indices, n_levels):
+            self.refine_batch([(q[0], q[1][level], q[2][level]) + tuple(q[3:]) for q in queries], max_wave_bytes)
+
+    @staticmethod
+    def _stack(pnp_points2D, references, point2D_idxs, inliers):
+        """correspondences that share a keypoint as ONE keypoint with several targets: (keypoints, targets, keypoint
+        indices, admitted, slot of every correspondence)"""
         if point2D_idxs is None:
             raise ValueError("point2D_idxs must not be None in stacked QKA.")
         slot_of, slots = {}, []                       # keypoint index -> position among the distinct keypoints
@@ -93,7 +130,12 @@ class QueryKeypointAdjuster:
             stacked_kps[where[k]] = pnp_points2D[k]
             targets[where[k]].append(ref)
             admitted[where[k]] = admitted[where[k]] or inliers is None or bool(inliers[k])
-        self.solver.run(stacked_kps, fmap, targets, patch_idxs=slots, inliers=None if inliers is None else admitted)
+        return stacked_kps, targets, slots, (None if inliers is None else admitted), where
+
+    def refine_stacked(self, pnp_points2D, fmap, references, point2D_idxs, inliers=None):
+        """correspondences that share a keypoint are stacked into ONE keypoint with several targets"""
+        stacked_kps, targets, slots, admitted, where = self._stack(pnp_points2D, references, point2D_idxs, inliers)
+        self.solver.run(stacked_kps, fmap, targets, patch_idxs=slots, inliers=admitted)
         for k, slot in enumerate(where):
             pnp_points2D[k] = stacked_kps[slot]
 
@@ -272,14 +314,47 @@ class QueryLocalizer:
         return self._localize_end(st)
 
     def localize_batch(self, queries, max_wave_bytes=0.0):
-        """localize() for every entry of `queries` (dicts of localize's keyword arguments): QKA and PnP per query as
-        localize runs them, then one batched QBA solve per feature level over every query that has a pose, then the
-        per-query inlier recomputation.  Returns the list of pose dicts localize would return."""
-        states = [self._localize_begin(**q) for q in queries]
+        """localize() for every entry of `queries` (dicts of localize's keyword arguments): per feature level the
+        reference selection of every query at once (one pxr_query_match_run for target_reference 'nearest', against the
+        level's stored observations packed once and kept in device memory), per level one batched QKA solve, PnP per
+        query, one batched QBA solve per level over every query that has a pose, then the per-query inlier
+        recomputation.  Returns the list of pose dicts localize would return."""
+        states = [self._localize_prepare(**q) for q in queries]
+        live = [st for st in states if "result" not in st]
+        if live and st_needs_features(live):
+            if self.conf.target_reference == "nearest":
+                per_level = [loc.find_nearest_references_batch(
+                    [(st["fmaps"][level], refs, st["points2D"], st["points3D_id"], st["point2D_idxs"]) for st in live],
+                    to_ctr(self.conf.interpolation), _table=self._observation_table(level))
+                    for level, refs in enumerate(self.references)]
+                for k, st in enumerate(live):
+                    st["references"] = [lvl[k] for lvl in per_level]
+            else:
+                for st in live:
+                    st["references"] = self.get_query_references(st["points3D_id"], st["fmaps"], st["points2D"],
+                                                                 st["point2D_idxs"])
+            for st in live:
+                if len(st["fmaps"]) != len(st["references"]):
+                    raise ValueError("one reference map per feature level is required")
+            if self.conf.QKA.apply:
+                self.query_keypoint_adjuster.refine_multilevel_batch(
+                    [(st["points2D"], st["fmaps"], st["references"], st["point2D_idxs"]) for st in live], max_wave_bytes)
+        states = [st if "result" in st else self._localize_pose(st) for st in states]
         live = [st for st in states if "result" not in st]
         if self.conf.QBA.apply and live:
             self.query_bundle_adjuster.refine_multilevel_batch([self._qba_args(st) for st in live], max_wave_bytes)
         return [st["result"] if "result" in st else self._localize_end(st) for st in states]
+
+    def _observation_table(self, level):
+        """every stored observation descriptor of the level's 3D points, packed once and kept in device memory:
+        (rows, {point id: (first row, count)})"""
+        cache = self.__dict__.setdefault("_obs_tables", {})
+        if level not in cache:
+            refs = self.references[level]
+            pids = [p for p in refs if getattr(refs[p], "observations", None)]
+            rows, where = loc.observation_table(refs, pids)
+            cache[level] = (_engine.device_array(rows) if len(rows) else rows, where)
+        return cache[level]
 
     @staticmethod
     def _qba_args(st):
@@ -290,6 +365,22 @@ class QueryLocalizer:
     def _localize_begin(self, keypoints, pnp_point2D_idxs, pnp_points3D_id, query_camera, image_path=None, query_fmaps=None,
                         pose_estimator=None):
         """localize up to the QBA step: {"result": pose dict} when it ends early, else the state _localize_end takes"""
+        st = self._localize_prepare(keypoints, pnp_point2D_idxs, pnp_points3D_id, query_camera, image_path, query_fmaps,
+                                    pose_estimator)
+        if "result" in st:
+            return st
+        if st_needs_features([st]):
+            st["references"] = self.get_query_references(st["points3D_id"], st["fmaps"], st["points2D"], st["point2D_idxs"])
+            if len(st["fmaps"]) != len(st["references"]):
+                raise ValueError("one reference map per feature level is required")
+        if self.conf.QKA.apply:
+            self.query_keypoint_adjuster.refine_multilevel(st["points2D"], st["fmaps"], st["references"],
+                                                           point2D_idxs=st["point2D_idxs"])
+        return self._localize_pose(st)
+
+    def _localize_prepare(self, keypoints, pnp_point2D_idxs, pnp_points3D_id, query_camera, image_path=None,
+                          query_fmaps=None, pose_estimator=None):
+        """the checks and inputs of one query: {"result": pose dict} when it ends early, else its state"""
         if len(pnp_point2D_idxs) != len(pnp_points3D_id):
             raise ValueError("one 3D point id per 2D index is required")
         if image_path is None and query_fmaps is None:
@@ -303,30 +394,30 @@ class QueryLocalizer:
         if query_fmaps is None and require_feats:
             query_fmaps = self._query_features(image_path, keypoints, sorted(set(pnp_point2D_idxs)))
         pnp_points2D = keypoints[pnp_point2D_idxs]           # a copy: QKA refines the correspondences' points
-        query_references = None
-        if require_feats:
-            query_references = self.get_query_references(pnp_points3D_id, query_fmaps, pnp_points2D, pnp_point2D_idxs)
-            if len(query_fmaps) != len(query_references):
-                raise ValueError("one reference map per feature level is required")
-        if self.conf.QKA.apply:
-            self.query_keypoint_adjuster.refine_multilevel(pnp_points2D, query_fmaps, query_references,
-                                                           point2D_idxs=pnp_point2D_idxs)
-        pose_dict = self._absolute_pose(pnp_points2D, pnp_points3D, query_camera, pose_estimator)
+        return {"camera": query_camera, "points2D": pnp_points2D, "points3D": pnp_points3D, "points3D_id": pnp_points3D_id,
+                "fmaps": query_fmaps, "references": None, "point2D_idxs": pnp_point2D_idxs, "require_feats": require_feats,
+                "pose_estimator": pose_estimator}
+
+    def _localize_pose(self, st):
+        """PnP on the (refined) correspondences and the inlier selection: {"result": pose dict} when PnP fails"""
+        pnp_points2D, pnp_points3D, query_camera = st["points2D"], st["points3D"], st["camera"]
+        pose_dict = self._absolute_pose(pnp_points2D, pnp_points3D, query_camera, st["pose_estimator"])
         if not pose_dict.get("success", False):
             return {"result": pose_dict}
         inliers = pose_dict.get("inliers", [True] * len(pnp_points3D))
         if self.conf.unique_inliers:                          # None / False: keep what PnP says
             if self.conf.unique_inliers == "random":
-                inliers = find_unique_inliers(pnp_points3D_id, pre_inliers=inliers)
+                inliers = find_unique_inliers(st["points3D_id"], pre_inliers=inliers)
             elif self.conf.unique_inliers == "min_error":
-                inliers = find_unique_min_reproj_inliers(pnp_points3D_id, pose_dict["qvec"], pose_dict["tvec"], query_camera,
+                inliers = find_unique_min_reproj_inliers(st["points3D_id"], pose_dict["qvec"], pose_dict["tvec"], query_camera,
                                                          pnp_points2D, self.reconstruction, pre_inliers=inliers,
-                                                         point2D_idxs=pnp_point2D_idxs)
+                                                         point2D_idxs=st["point2D_idxs"])
             else:
                 from .. import logger
                 logger.warning("Unknown unique_inlier method %s.", self.conf.unique_inliers)
         return {"pose": pose_dict, "camera": query_camera, "points2D": pnp_points2D, "points3D": pnp_points3D,
-                "fmaps": query_fmaps, "references": query_references, "inliers": inliers, "point2D_idxs": pnp_point2D_idxs}
+                "fmaps": st["fmaps"], "references": st["references"], "inliers": inliers,
+                "point2D_idxs": st["point2D_idxs"]}
 
     def _localize_end(self, st):
         pose_dict = st["pose"]
