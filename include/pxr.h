@@ -515,6 +515,23 @@ int pxr_extract_patches(pxr_ctx* ctx, const void* dense, int32_t dense_on_device
                         int32_t height, int32_t width, int32_t channels_first, const int32_t* corners, int64_t n_patches,
                         int32_t patch_size, int32_t l2_normalize, int32_t out_dtype, void* out_host, void** out_device);
 
+/* ---- dense SIFT -> patch slab ----------------------------------------------
+ * replaces the reference's `dsift` model (features/models/dsift.py: kornia's DenseSIFTDescriptor, stride 1, padding 1)
+ * followed by the sparse branch of FeatureExtractor.tensor_to_fmap: the descriptor map of a grayscale image, each
+ * pixel's C = num_ang_bins * num_spatial_bins^2 channels clipped, rootsift-mapped, optionally L2-normalised and cast,
+ * computed by one fused kernel only where it is asked for.  The map is H' x W' with
+ * H' = height + 2 (b / 2) - b + 1 + 3 - num_spatial_bins (b = spatial_bin_size), likewise W'.  Kornia parity is unverified.
+ *  image      [height][width] uint8, host or device memory
+ *  corners    host [n][2] (x0, y0) in map coordinates, every window inside the map: the slab [n][ps][ps][C];
+ *             NULL: the whole map [H'][W'][C] (n_patches and patch_size are ignored).  A window of the slab is bit for bit
+ *             the same window of the map.
+ *  supported  num_ang_bins 4 or 8, num_spatial_bins 2 or 4, spatial_bin_size 1..8 (otherwise PXR_ERR_UNSUPPORTED)
+ *  out_host / out_device as for pxr_extract_patches */
+int pxr_dsift(pxr_ctx* ctx, const uint8_t* image, int32_t image_on_device, int32_t height, int32_t width,
+              int32_t num_ang_bins, int32_t num_spatial_bins, int32_t spatial_bin_size, float clipval, int32_t rootsift,
+              int32_t l2_normalize, const int32_t* corners, int64_t n_patches, int32_t patch_size, int32_t out_dtype,
+              void* out_host, void** out_device);
+
 /* ---- featuremetric KA ---------------------------------------------------
  * replaces _keypoint_adjustment.FeatureMetricKeypointOptimizer.run
  * (keypoint_adjustment/bindings.cc:17-34; featuremetric_keypoint_optimizer.h:50-202;

@@ -483,6 +483,46 @@ def extract_patches(dense, corners, patch_size, l2_normalize=True, out_dtype=np.
     return out if to_host else DeviceSlab(dptr.value, (n, patch_size, patch_size, ch), out_dtype, ctx)
 
 
+def dsift_map_size(height, width, num_spatial_bins=4, spatial_bin_size=4):
+    """(H', W') of the dense SIFT map of a height x width image (stride 1, padding 1, as the reference's dsift model)"""
+    extra = 2 * (spatial_bin_size // 2) - spatial_bin_size + 1 + 3 - num_spatial_bins
+    return height + extra, width + extra
+
+
+def dsift(image, corners=None, patch_size=16, num_ang_bins=8, num_spatial_bins=4, spatial_bin_size=4, clipval=0.2,
+          rootsift=True, l2_normalize=True, out_dtype=np.float16, to_host=False, ctx=None):
+    """pxr_dsift: dense SIFT of ONE [H,W] uint8 grayscale image (a host numpy array or anything with
+    __cuda_array_interface__).  With `corners` [n,2] (x0, y0) in map coordinates -> the windows [n, ps, ps, C]; without
+    -> the whole map [1, H', W', C].  A DeviceSlab, or a numpy array with to_host=True."""
+    ctx = ctx or _capi.default_context()
+    cai = getattr(image, "__cuda_array_interface__", None)
+    if cai is not None:
+        if cai.get("strides") is not None:
+            raise ValueError("the image must be contiguous")
+        shape, in_dtype, ptr, on_dev = tuple(cai["shape"]), np.dtype(cai["typestr"]), int(cai["data"][0]), 1
+    else:
+        image = np.ascontiguousarray(image)
+        shape, in_dtype, ptr, on_dev = image.shape, image.dtype, image.ctypes.data, 0
+    if len(shape) != 2 or in_dtype != np.uint8 or np.dtype(out_dtype) not in _capi.DTYPE_IDS:
+        raise ValueError("an image is a [H,W] uint8 array and the output float16/32/64")
+    h, w = shape
+    ch = num_ang_bins * num_spatial_bins ** 2
+    if corners is None:
+        out_shape, c_corners, n = (1,) + dsift_map_size(h, w, num_spatial_bins, spatial_bin_size) + (ch,), None, 0
+    else:
+        c_corners = np.ascontiguousarray(corners, np.int32).reshape(-1, 2)
+        n = len(c_corners)
+        out_shape = (n, patch_size, patch_size, ch)
+    out = np.zeros(out_shape, out_dtype) if to_host else None
+    dptr = C.c_void_p()
+    _capi.check(ctx.lib.pxr_dsift(ctx.handle, C.c_void_p(ptr), on_dev, int(h), int(w), int(num_ang_bins),
+                                  int(num_spatial_bins), int(spatial_bin_size), C.c_float(clipval), int(bool(rootsift)),
+                                  int(bool(l2_normalize)), _p(c_corners), C.c_int64(n), int(patch_size),
+                                  _capi.DTYPE_IDS[np.dtype(out_dtype)], _p(out) if to_host else None,
+                                  None if to_host else C.byref(dptr)))
+    return out if to_host else DeviceSlab(dptr.value or 0, out_shape, out_dtype, ctx)
+
+
 def interpolate_patches(patches, corners, scales, item_patch, xys, interp=None, upsampling_factor=1.0, ctx=None):
     """pxr_interpolate_descriptors: the (bicubic, optionally L2-normalised) descriptor of patch item_patch[i] of a host
     [N,H,W,C] patch array at IMAGE coordinates xys[i] -> [n_items, C] float64"""

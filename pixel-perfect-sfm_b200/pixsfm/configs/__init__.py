@@ -1,6 +1,7 @@
 """Named configuration presets (the reference ships them as YAML files in pixsfm/configs/ and resolves names with
 `parse_config_path`, configs/__init__.py:8-26).  Here a preset is a function returning the nested dict; a path to a YAML
 file — the reference's own files included — is accepted wherever a preset name is."""
+from copy import deepcopy
 from pathlib import Path
 
 from .. import defaults
@@ -30,7 +31,25 @@ def _norefine():
     return {"mapping": {"KA": dict(apply=False), "BA": dict(apply=False)}}
 
 
-default_configs = {"default": _default, "low_memory": _low_memory, "norefine": _norefine}
+def _dsift():
+    """dense SIFT features computed here (features/models/dsift.py): PixSfM and QueryLocalizer run from images"""
+    dense = dict(model=dict(name="dsift", rootsift=True, spatial_bin_size=4), sparse=True, use_cache=False, max_edge=2000,
+                 patch_size=16, device="cuda", dtype="half")
+    ka = dict(apply=True, strategy="featuremetric", level_indices=None, max_kps_per_problem=50,
+              optimizer=dict(print_summary=False, bound=4.0))
+    ba = dict(apply=True, strategy="feature_reference", repeats=1, level_indices=None,
+              optimizer=dict(solver=dict(max_num_iterations=10), print_summary=False, refine_focal_length=False,
+                             refine_extra_params=False, refine_extrinsics=False))
+    qka = dict(apply=True, level_indices=None, feature_inlier_thresh=-1, optimizer=dict(print_summary=False))
+    qba = dict(apply=True, level_indices=None,
+               optimizer=dict(print_summary=False, refine_focal_length=False, refine_extra_params=False))
+    return {"dense_features": dense,
+            "mapping": {"dense_features": deepcopy(dense), "KA": ka, "BA": ba},
+            "localization": {"dense_features": deepcopy(dense), "target_reference": "nearest", "unique_inliers": "min_error",
+                             "overwrite_features_sparse": False, "QKA": qka, "QBA": qba}}
+
+
+default_configs = {"default": _default, "low_memory": _low_memory, "norefine": _norefine, "dsift": _dsift}
 
 
 def parse_config_path(name_or_path):

@@ -4,8 +4,10 @@ The reference's FeatureExtractor (pixsfm/features/extractor.py) owns the CNN (S2
 `tensor_to_fmap` (:152-236): L2-normalise the C-channel map, cast it, and either keep it dense or cut one
 `patch_size` x `patch_size` patch per keypoint with `corner = clip(int(kp * scale - ps / 2), 0, [w, h] - ps - 1)`.  The CNN
 is not part of this package; the step after it is, so that any model — a callable image name -> list of [C,H,W] maps,
-finest level first — plugs into `PixSfM(conf, extractor=DenseFeatureExtractor(model, ...))`."""
+finest level first — plugs into `PixSfM(conf, extractor=DenseFeatureExtractor(model, ...))`.  The one model the package
+computes itself, dense SIFT, has the reference's `FeatureExtractor(conf)`: images in, FeatureManager out."""
 import os
+from pathlib import Path
 
 import numpy as np
 
@@ -21,16 +23,17 @@ def _as_numpy(x):
     return np.asarray(x)
 
 
-def _map_shape(x):
-    cai = getattr(x, "__cuda_array_interface__", None)
-    return tuple(cai["shape"]) if cai is not None else np.shape(x)
-
-
 def patch_corners(keypoints, scale, patch_size, map_wh):
     """top-left map pixel of every keypoint's patch (extractor.py:192-193): truncation towards zero, then clamped so
     that the patch and one more pixel stay inside the map"""
     corners = (np.asarray(keypoints, np.float64) * scale - patch_size / 2.0).astype(np.int32)
     return np.clip(corners, [0, 0], np.asarray(map_wh, np.int64) - patch_size - 1).astype(np.int32)
+
+
+def sparse_pays_off(map_h, map_w, n_keypoints, patch_size):
+    """the reference's rule (tensor_to_fmap, features/extractor.py:182-187): patches are kept only while they are smaller
+    than the map they are cut from"""
+    return map_h * map_w > n_keypoints * patch_size * patch_size
 
 
 def cut_patches(dense_hwc, corners, patch_size):
@@ -62,7 +65,7 @@ def dense_to_fmap_on_device(featuremap, image_size, keypoints, keypoint_ids=None
     source = featuremap if cai is not None else _as_numpy(featuremap)
     if cai is None and source.ndim == 4:
         source = source[0]
-    if h * w <= len(keypoints) * patch_size * patch_size:
+    if not sparse_pays_off(h, w, len(keypoints), patch_size):
         # sparse does not pay off (reference tensor_to_fmap, features/extractor.py:182-187, same rule as dense_to_fmap):
         # ONE dense patch, normalised / cast / transposed to HWC by the same gather kernel with a single h x w window.
         # pxr_extract_patches takes square windows, so a non-square map goes through the host path.
@@ -97,10 +100,10 @@ def dense_to_fmap(featuremap, image_size, keypoints=None, keypoint_ids=None, pat
     if l2_normalize:
         hwc = hwc / np.maximum(np.linalg.norm(hwc.astype(np.float32), axis=-1, keepdims=True), 1e-12)   # F.normalize eps
     hwc = np.ascontiguousarray(hwc, dtype=dtype)
-    h, w, c = hwc.shape
+    h, w = hwc.shape[:2]
     scale = np.array((w / image_size[0], h / image_size[1]))
     # sparse only pays off while the patches are smaller than the map they are cut from
-    if sparse and hwc.size > len(keypoints) * patch_size * patch_size * c:
+    if sparse and sparse_pays_off(h, w, len(keypoints), patch_size):
         corners = patch_corners(keypoints, scale, patch_size, (w, h))
         return features.FeatureMap(cut_patches(hwc, corners, patch_size), keypoint_ids, corners,
                                    {"scale": scale, "is_sparse": True, "patch_size": patch_size})
@@ -149,17 +152,11 @@ class DenseFeatureExtractor:
                 if req_keypoint_ids is not None:
                     ids = [int(i) for i in req_keypoint_ids[name]]
                     kps = kps[ids]
-            maps = self.model(name)
+            made = self._image_fmaps(image_dir, name, kps, ids)
             if manager is None:
-                manager = features.FeatureManager([_map_shape(m)[-3] for m in maps], _DTYPES[self.conf["dtype"]])
-            for level, fmap in enumerate(maps):
-                if self.conf["on_device"] and self.conf["sparse"] and kps is not None:
-                    made = dense_to_fmap_on_device(fmap, self.image_size(name), kps, ids, self.conf["patch_size"],
-                                                   self.conf["l2_normalize"], _DTYPES[self.conf["dtype"]])
-                else:
-                    made = dense_to_fmap(fmap, self.image_size(name), kps, ids, self.conf["patch_size"], self.conf["sparse"],
-                                         self.conf["l2_normalize"], _DTYPES[self.conf["dtype"]])
-                manager.fset(level).emplace(name, made)
+                manager = features.FeatureManager([m.channels for m in made], _DTYPES[self.conf["dtype"]])
+            for level, fmap in enumerate(made):
+                manager.fset(level).emplace(name, fmap)
         if manager is None:
             raise ValueError("no image to extract features for")
         if use_cache:
@@ -167,6 +164,22 @@ class DenseFeatureExtractor:
             store_features.write_feature_manager_cache(cache_path, manager, self.conf["cache_format"], level_prefix)
             return store_features.load_features_from_cache(cache_path, bool(self.conf["load_cache_on_init"]), level_prefix)
         return manager
+
+    def _image_fmaps(self, image_dir, name, kps, ids):
+        """one FeatureMap per level of image `name`: the patches around `kps` (ids `ids`) or the dense map"""
+        out = []
+        for fmap in self.model(name):
+            if self._on_device(kps):
+                out.append(dense_to_fmap_on_device(fmap, self.image_size(name), kps, ids, self.conf["patch_size"],
+                                                   self.conf["l2_normalize"], _DTYPES[self.conf["dtype"]]))
+            else:
+                out.append(dense_to_fmap(fmap, self.image_size(name), kps, ids, self.conf["patch_size"], self.conf["sparse"],
+                                         self.conf["l2_normalize"], _DTYPES[self.conf["dtype"]]))
+        return out
+
+    def _on_device(self, kps):
+        """the patches stay in device memory: asked for, and sparse patches are what is made"""
+        return bool(self.conf["on_device"] and self.conf["sparse"] and kps is not None)
 
     def features_from_graph(self, image_dir, graph, keypoints, cache_path=None):
         """patches for the keypoints that take part in a match (reference extract.py:197-215)"""
@@ -188,3 +201,78 @@ class DenseFeatureExtractor:
             kps[[k for k, _ in seen]] = world_to_image(cam.model_id, cam.params, image.qvec, image.tvec, xyz)
             names.append(image.name); keypoints[image.name] = kps; ids[image.name] = [k for k, _ in seen]
         return self.features_from_image_list(image_dir, names, keypoints, ids, cache_path)
+
+
+class FeatureExtractor(DenseFeatureExtractor):
+    """The reference's FeatureExtractor (features/extractor.py:28-236) for the model this package computes itself, dense
+    SIFT (`model: {name: dsift}`, features/models/dsift.py).  Each image is opened with PIL, resized per pyramid scale to
+    `round(min(max_edge / max(w, h), 1) * size * scale)` with the `resize` filter and converted to grayscale ("L", what
+    torchvision's Grayscale does); each scale gives one feature level.  Sparse features come from the fused kernel at the
+    keypoints' windows only, dense ones from the same kernel over the whole map.  Cache, `on_device` and the
+    sparse-or-dense rule are DenseFeatureExtractor's.  The CNN models (S2DNet, VGG) need downloaded weights and are not
+    part of this package."""
+    default_conf = dict(DenseFeatureExtractor.default_conf, device="auto", fast_image_load=False, max_edge=1600,
+                        model={"name": "s2dnet"}, pyr_scales=[1.0], resize="LANCZOS")
+    filters = ("BILINEAR", "BICUBIC", "LANCZOS")
+
+    def __init__(self, conf=None):
+        conf = dict(conf or {})
+        model_conf = dict(conf.get("model") or self.default_conf["model"])
+        super().__init__(None, None, conf)
+        self.conf["model"] = model_conf
+        if model_conf.get("name") != "dsift":
+            raise ValueError("dense feature model %r is not part of this package: only 'dsift' is computed here; the CNN "
+                             "models (s2dnet, vgg) need downloaded weights — pass their FeatureManager or a "
+                             "DenseFeatureExtractor around them" % (model_conf.get("name"),))
+        if self.conf["device"] not in ("auto", "cuda"):
+            raise ValueError("dense SIFT runs on the GPU only (device %r)" % (self.conf["device"],))
+        if self.conf["resize"] not in self.filters:
+            raise ValueError("resize must be one of %s" % (self.filters,))
+        if not self.conf["pyr_scales"] or any(float(s) <= 0 for s in self.conf["pyr_scales"]):
+            raise ValueError("pyr_scales must be a non-empty list of positive scales")
+        from .models import DSIFT
+        self.model = DSIFT(model_conf)
+        self.channels_per_level = list(self.model.output_dims) * len(self.conf["pyr_scales"])
+
+    def get_scaled_image_size(self, image, pyr_scale=1.0):
+        w, h = image.size
+        return [int(round(min(self.conf["max_edge"] / max(w, h), 1) * x * pyr_scale)) for x in (w, h)]
+
+    def load_image(self, path):
+        """-> ([one [h, w] uint8 grayscale image per pyramid scale], (width, height) of the file)"""
+        import PIL.Image
+        image = PIL.Image.open(path)
+        size = image.size
+        if self.conf["fast_image_load"]:
+            image.draft("RGB", self.get_scaled_image_size(image, self.conf["pyr_scales"][0]))
+        levels = []
+        for pyr_scale in self.conf["pyr_scales"]:
+            resized = image.resize(tuple(self.get_scaled_image_size(image, pyr_scale)),
+                                   getattr(PIL.Image, self.conf["resize"]))
+            levels.append(np.ascontiguousarray(np.asarray(resized.convert("L"), np.uint8)))
+        return levels, size
+
+    def _image_fmaps(self, image_dir, name, kps, ids):
+        path = name if image_dir is None else Path(image_dir) / name
+        images, size = self.load_image(path)
+        ps, sparse = self.conf["patch_size"], self.conf["sparse"]
+        if sparse and kps is None:
+            raise RuntimeError("Cannot run sparse feature extraction without any keypoints.")
+        if kps is not None:
+            kps = np.asarray(kps, np.float64).reshape(-1, 2)
+            ids = list(range(len(kps))) if ids is None else ids
+        out = []
+        for image in images:
+            h, w = self.model.map_size(*image.shape)
+            scale = np.array((w / size[0], h / size[1]))
+            run = dict(patch_size=ps, l2_normalize=self.conf["l2_normalize"], dtype=self.conf["dtype"],
+                       to_host=not self._on_device(kps))
+            if sparse and sparse_pays_off(h, w, len(kps), ps):
+                corners = patch_corners(kps, scale, ps, (w, h))
+                out.append(features.FeatureMap(self.model(image, corners, **run), ids, corners,
+                                               {"scale": scale, "is_sparse": True, "patch_size": ps}))
+            else:
+                out.append(features.FeatureMap(self.model(image, None, **run), [features.kDenseId],
+                                               np.zeros((1, 2), np.int32),
+                                               {"scale": scale, "is_sparse": False, "patch_size": ps}))
+        return out

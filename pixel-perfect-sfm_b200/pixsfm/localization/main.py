@@ -221,13 +221,18 @@ class QueryLocalizer:
             from ..refine_colmap import _load_conf
             conf = _load_conf(conf)
         if isinstance(conf, dict) and isinstance(conf.get("localization"), dict):
-            conf = conf["localization"]
+            from ..refine_colmap import _resolve_references
+            conf = _resolve_references(conf["localization"], conf)
         self.conf = merge(self.default_conf, conf or {})
         if self.conf.QKA.stack_correspondences and self.conf.target_reference not in ("nearest", "robust_mean"):
             raise ValueError("Stacked QKA requires a np.ndarray reference for each 2D-3D correspondence. Consider setting "
                              "target_references to 'nearest' or 'robust_mean'.")
         self.query_keypoint_adjuster = QueryKeypointAdjuster(to_ctr(self.conf.QKA))
         self.query_bundle_adjuster = QueryBundleAdjuster(to_ctr(self.conf.QBA))
+        from ..refine_colmap import _model_name
+        if extractor is None and _model_name(self.conf.dense_features) == "dsift":
+            from ..features.extractor import FeatureExtractor
+            extractor = FeatureExtractor(to_ctr(self.conf.dense_features))
         self.extractor = extractor
         self.pose_estimator = pose_estimator
         self.reference_extractor = ba.ReferenceExtractor(to_ctr(self.conf.references), to_ctr(self.conf.interpolation))

@@ -2,7 +2,9 @@
 COLMAP database -> keypoint adjustment -> database, COLMAP model -> bundle adjustment -> model.
 
 What differs from the reference, and why:
-  * dense feature extraction (the S2DNet CNN, `features/extractor.py`) is not part of this package: pass an `extractor`
+  * dense features: with `dense_features.model.name == "dsift"` (the `dsift` preset) the driver builds the package's
+    own `features.extractor.FeatureExtractor`, which computes dense SIFT on the GPU, and runs from an image directory.
+    The CNN models (S2DNet, VGG) need downloaded weights and are not part of this package: for them pass an `extractor`
     object with the reference's interface (`extract.features_from_graph` / `features_from_reconstruction` are called
     on it) or hand the adjusters a ready `feature_manager`.  Without either the call raises — nothing is faked.
   * models are read and written by `util.colmap_model_io` (pycolmap is not installable offline); pycolmap
@@ -21,7 +23,7 @@ from .bundle_adjustment import BundleAdjuster
 from .keypoint_adjustment import KeypointAdjuster, build_matching_graph
 from .util.colmap import read_keypoints_from_db, read_matches_from_db, write_keypoints_to_db
 from .util.colmap_types import Reconstruction
-from .util.conf import merge, to_conf
+from .util.conf import merge, to_conf, to_ctr
 
 
 def _load_conf(conf):
@@ -58,6 +60,12 @@ def _resolve_references(node, top):
     return out
 
 
+def _model_name(dense_features):
+    """dense_features.model.name, or None"""
+    model = dense_features.get("model") if isinstance(dense_features, dict) else None
+    return model.get("name") if isinstance(model, dict) else None
+
+
 class PixSfM:
     default_conf = {
         "interpolation": interpolation_default_conf,
@@ -81,6 +89,9 @@ class PixSfM:
         for part in ("KA", "BA"):       # "${..interpolation}": the shared block unless the adjuster has its own
             if "interpolation" not in conf.get(part, {}):
                 self.conf[part]["interpolation"] = to_conf(deepcopy(interpolation))
+        if extractor is None and _model_name(self.conf["dense_features"]) == "dsift":
+            from .features.extractor import FeatureExtractor
+            extractor = FeatureExtractor(to_ctr(self.conf["dense_features"]))
         self.extractor = extractor
         # the reference builds its extractor FROM conf.dense_features (refine_colmap.py:52-56); here the extractor comes in
         # from outside (the CNN is not part of this package), so the block is applied to it where it knows the option

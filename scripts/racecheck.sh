@@ -1,6 +1,6 @@
 #!/bin/bash
 # compute-sanitizer racecheck (shared-memory hazards) over the kernels that use shared memory: K1 (TMA ring + aux),
-# the persistent Cholesky (tiles, named barriers), the KA kernel (dense H / vectors), IRLS.
+# the persistent Cholesky (tiles, named barriers), the KA kernel (dense H / vectors), IRLS, dense SIFT (staged halo, E / P).
 set -u
 run() {
   echo "=== $*"
@@ -9,3 +9,4 @@ run() {
 run tests/test_gpu_ba_parity.py -k "residual_blocks or tile_dag"
 run tests/test_gpu_ka.py -k "matches_oracle"
 run tests/test_gpu_refs.py
+run tests/test_gpu_dsift.py -k "oracle or bit_for_bit"
