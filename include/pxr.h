@@ -651,6 +651,93 @@ int pxr_qba_plan_waves(const pxr_qba_desc* desc, int32_t* wave_begin, int32_t* n
 int pxr_qba_debug_linearize(pxr_ctx* ctx, const pxr_qba_desc* desc, const pxr_interp_config* interp,
                             const pxr_solver_options* opt, double* cost, double* H, double* g, double* xy, double* rec);
 
+/* ---- batched absolute pose estimation ------------------------------------------
+ * pycolmap 0.4's absolute_pose_estimation (COLMAP 3.8 EstimateAbsolutePose + RefineAbsolutePose) for N independent
+ * queries: LO-RANSAC over P3P minimal samples (Lambda Twist), then a Cauchy-robust LM refinement of the pose (and,
+ * when asked, of the focal length / extra parameters) over the RANSAC inliers.  One CTA estimates one query
+ * (csrc/pxr_pnp.cu); a query's results depend only on its own inputs and seed, never on the other queries of the call.
+ *
+ * RANSAC, precisely (tests restate it on the host and draw the same samples):
+ *  - every 2D point goes once to the normalised image plane (ImageToWorld); thr = max_error / mean focal length; the
+ *    residual of a correspondence under (R, t) is, with (x, y, z) = R X + t (sums left to right, no fused
+ *    multiply-add) and iz = 1 / z, (x iz - u)^2 + (y iz - v)^2; it is an inlier when z > DBL_EPSILON and the residual
+ *    <= thr^2.  Support = (number of inliers, sum of their residuals): more inliers wins, then the smaller sum, then
+ *    the lower (trial, solution) index.
+ *  - trials run in rounds of PXR_PNP_ROUND_TRIALS; trial t of a query with n correspondences draws words
+ *    w_d = splitmix64(splitmix64(seed) ^ (t << 8) ^ d), d = 0, 1, ... 63, takes index ((w_d >> 32) * n) >> 32 from
+ *    each and keeps the first three distinct ones (fewer than three after 64 draws: the trial has no hypothesis);
+ *    splitmix64(x): z = x + 0x9E3779B97F4A7C15, z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9,
+ *    z = (z ^ z >> 27) * 0x94D049BB133111EB, z ^ z >> 31 (mod 2^64).  Trials t >= max_num_trials are not run.
+ *  - P3P gives up to four hypotheses per trial, solution s of trial t has index 4 t + s; after a round the best
+ *    hypothesis of the round replaces the best so far when its support is better, and then, when it has more than 3
+ *    inliers, local optimisation runs: 3 Gauss-Newton steps on the 6-dof pose over that hypothesis' inliers in the
+ *    normalised plane, kept when its support is better still.  (COLMAP's LO-RANSAC re-estimates with EPnP there.)
+ *  - after every round the required trial count is COLMAP's ceil(log(1 - confidence) / log(1 - ratio^3) *
+ *    dyn_num_trials_multiplier), ratio = inliers / n, clamped to [min_num_trials, max_num_trials]; the query stops when
+ *    the trials run reach it, so up to PXR_PNP_ROUND_TRIALS - 1 trials more than COLMAP's can run.
+ *  - success: n >= 3 and the best support has >= 3 inliers and inliers / n >= min_inlier_ratio. */
+#define PXR_PNP_ROUND_TRIALS 128
+
+typedef struct {
+  int32_t n_queries;
+  const int64_t* corr_begin;      /* [n_queries+1] non-decreasing from 0: query q owns correspondences
+                                     [corr_begin[q], corr_begin[q+1]) */
+  const double* points2D;         /* [n_corr][2] pixels, COLMAP convention (pixel centres at +0.5) */
+  const double* points3D;         /* [n_corr][3] */
+  const int32_t* cam_model;       /* [n_queries] pxr_camera_model */
+  double* cam_params;             /* [n_queries][PXR_MAX_CAM_PARAMS] in/out: written only when refinement refines
+                                     intrinsics and the query succeeds */
+  const uint64_t* seed;           /* [n_queries] */
+  double* qvec;                   /* [n_queries][4] out (w,x,y,z) world->camera, written when the query succeeds */
+  double* tvec;                   /* [n_queries][3] out */
+  uint8_t* inlier_mask;           /* [n_corr] out: inliers of the returned pose (recomputed after refinement) */
+} pxr_pnp_desc;
+
+typedef struct {
+  /* AbsolutePoseEstimationOptions / RANSACOptions */
+  double max_error;               /* pixels */
+  double min_inlier_ratio;
+  int32_t min_num_trials, max_num_trials;
+  double confidence;
+  double dyn_num_trials_multiplier;
+  int32_t estimate_focal_length;  /* must be 0 (PXR_ERR_UNSUPPORTED) */
+  /* AbsolutePoseRefinementOptions */
+  int32_t refine;                 /* 0: return the RANSAC pose */
+  double gradient_tolerance;
+  int32_t max_num_iterations;
+  double loss_function_scale;     /* Cauchy */
+  int32_t refine_focal_length, refine_extra_params;
+  /* ceres' function / parameter tolerances, which COLMAP leaves at 1e-6 / 1e-8 (pycolmap has no name for them) */
+  double function_tolerance, parameter_tolerance;
+} pxr_pnp_options;
+
+typedef struct {
+  int32_t status;                 /* PXR_OK, or PXR_ERR_NUMERIC: refinement's initial cost not finite (pose and camera
+                                     untouched, success 0) */
+  int32_t success;
+  int32_t num_inliers;            /* of the returned pose */
+  int32_t num_trials;             /* RANSAC trials run */
+  int32_t best_trial, best_solution;   /* the winning hypothesis (-1 when none) */
+  int32_t local_optimized;        /* the winner is its local optimisation */
+  int32_t num_iterations;         /* refinement: as pxr_qba_result */
+  int32_t termination_type;
+  double initial_cost, final_cost;
+} pxr_pnp_result;
+
+/* Fills opt with pycolmap 0.4's defaults (max_error 12 px). */
+void pxr_default_pnp_options(pxr_pnp_options* opt);
+/* Estimates every query in one launch of the RANSAC kernel and one of the refinement kernel.  results [n_queries];
+ * total (or NULL): kernel time, h2d_bytes, kernel launches, message.  Arguments are checked before the context: a
+ * NULL or malformed desc, a non-monotone corr_begin and an unknown camera model are PXR_ERR_INVALID_ARGUMENT /
+ * PXR_ERR_UNSUPPORTED without a device; so is estimate_focal_length != 0 (PXR_ERR_UNSUPPORTED). */
+int pxr_pnp_run(pxr_ctx* ctx, const pxr_pnp_desc* desc, const pxr_pnp_options* opt, pxr_pnp_result* results,
+                pxr_summary* total);
+/* Device code on its own (tests): ImageToWorld of n pixels xy [n][2] -> out [n][2]; P3P of n triplets of normalised
+ * image points x [n][3][2] and world points X [n][3][3] -> poses [n][4][7] (qvec with w >= 0, tvec) and n_sol [n]. */
+int pxr_pnp_debug_image_to_world(pxr_ctx* ctx, int32_t model, const double* params, int64_t n, const double* xy,
+                                 double* out);
+int pxr_pnp_debug_p3p(pxr_ctx* ctx, int64_t n, const double* x, const double* X, double* poses, int32_t* n_sol);
+
 /* ---- batched query keypoint adjustment ------------------------------------------
  * replaces a loop of _localization.QueryKeypointOptimizer.run: N independent queries, each one problem of pxr_ka_run's
  * query mode (every residual block = one keypoint against one fixed descriptor).  One CTA solves one query; the

@@ -392,6 +392,61 @@ PYBIND11_MODULE(_pxr_pybind, m) {
     return py::dict("results"_a = out, "n_waves"_a = n_waves, "h2d_bytes"_a = s.h2d_bytes, "solve_time_s"_a = s.solve_time_s,
                     "total_time_s"_a = s.total_time_s);
   }, "ctx"_a, "problem"_a, "interpolation"_a = py::dict(), "options"_a = py::dict());
+  // batched absolute pose estimation: per query corr_begin [nq+1], cam_model, cam_params [nq,12] (in/out), seed [nq]
+  // (uint64), qvec [nq,4] / tvec [nq,3] (written for successful queries); per correspondence points2D [n,2],
+  // points3D [n,3], inlier_mask [n] (uint8, written); `options` takes pxr_pnp_options' field names
+  m.def("pnp_run", [](Context& ctx, py::dict problem, py::dict options) {
+    Fields f{problem, {}};
+    pxr_pnp_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.n_queries = (int32_t)f.len("cam_model");
+    d.cam_model = f.arr<int32_t>("cam_model");
+    d.cam_params = f.inout<double>("cam_params");
+    d.seed = f.arr<uint64_t>("seed");
+    d.qvec = f.inout<double>("qvec");
+    d.tvec = f.inout<double>("tvec");
+    d.corr_begin = f.arr<int64_t>("corr_begin");
+    if (f.len("corr_begin") != (int64_t)d.n_queries + 1) throw py::value_error("corr_begin must hold n_queries + 1 entries");
+    d.points2D = f.arr<double>("points2D", false);
+    d.points3D = f.arr<double>("points3D", false);
+    d.inlier_mask = f.inout<uint8_t>("inlier_mask");
+    pxr_pnp_options o; pxr_default_pnp_options(&o);
+    for (auto item : options) {
+      const std::string k = py::str(item.first);
+      py::handle v = item.second;
+      if (k == "max_error") o.max_error = v.cast<double>();
+      else if (k == "min_inlier_ratio") o.min_inlier_ratio = v.cast<double>();
+      else if (k == "min_num_trials") o.min_num_trials = v.cast<int32_t>();
+      else if (k == "max_num_trials") o.max_num_trials = v.cast<int32_t>();
+      else if (k == "confidence") o.confidence = v.cast<double>();
+      else if (k == "dyn_num_trials_multiplier") o.dyn_num_trials_multiplier = v.cast<double>();
+      else if (k == "estimate_focal_length") o.estimate_focal_length = v.cast<bool>();
+      else if (k == "refine") o.refine = v.cast<bool>();
+      else if (k == "gradient_tolerance") o.gradient_tolerance = v.cast<double>();
+      else if (k == "max_num_iterations") o.max_num_iterations = v.cast<int32_t>();
+      else if (k == "loss_function_scale") o.loss_function_scale = v.cast<double>();
+      else if (k == "refine_focal_length") o.refine_focal_length = v.cast<bool>();
+      else if (k == "refine_extra_params") o.refine_extra_params = v.cast<bool>();
+      else if (k == "function_tolerance") o.function_tolerance = v.cast<double>();
+      else if (k == "parameter_tolerance") o.parameter_tolerance = v.cast<double>();
+      else throw py::value_error("unknown pnp option '" + k + "'");
+    }
+    std::vector<pxr_pnp_result> res((size_t)std::max(d.n_queries, 1));
+    pxr_summary s; std::memset(&s, 0, sizeof(s));
+    int rc;
+    { py::gil_scoped_release nogil; rc = pxr_pnp_run(ctx.h, &d, &o, res.data(), &s); }
+    check(rc);
+    py::list out;
+    for (int q = 0; q < d.n_queries; ++q) {
+      const pxr_pnp_result& r = res[q];
+      out.append(py::dict("status"_a = r.status, "success"_a = (bool)r.success, "num_inliers"_a = r.num_inliers,
+                          "num_trials"_a = r.num_trials, "best_trial"_a = r.best_trial, "best_solution"_a = r.best_solution,
+                          "local_optimized"_a = (bool)r.local_optimized, "num_iterations"_a = r.num_iterations,
+                          "termination_type"_a = r.termination_type, "initial_cost"_a = r.initial_cost,
+                          "final_cost"_a = r.final_cost));
+    }
+    return py::dict("results"_a = out, "solve_time_s"_a = s.solve_time_s, "total_time_s"_a = s.total_time_s);
+  }, "ctx"_a, "problem"_a, "options"_a = py::dict());
   // batched query KA (a loop of QueryKeypointOptimizer.run): per query kp_begin [nq+1], patches_are_sparse [nq] and
   // one host patch block (`patch_blocks`, `corner` / `scale` back to back); per keypoint keypoints [n,2] (refined IN
   // PLACE), kp_patch (within its query's block) and desc_begin [n+1] into descs [m, C]

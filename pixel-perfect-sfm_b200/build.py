@@ -6,7 +6,10 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["pxr_api.cu", "pxr_upload.cu", "pxr_ba.cu", "pxr_ba_block.cu", "pxr_refs.cu", "pxr_ka.cu", "pxr_synth.cu", "pxr_extract.cu", "pxr_dsift.cu", "pxr_problem.cu", "pxr_qba.cu"]
+SOURCES = ["pxr_api.cu", "pxr_upload.cu", "pxr_ba.cu", "pxr_ba_block.cu", "pxr_refs.cu", "pxr_ka.cu", "pxr_synth.cu", "pxr_extract.cu", "pxr_dsift.cu", "pxr_problem.cu", "pxr_qba.cu", "pxr_pnp.cu"]
+# absolute pose estimation evaluates P3P and its residuals exactly as written, so that a host restatement in IEEE
+# double reproduces them bit for bit (tests/pnp_reference.py)
+FILE_FLAGS = {"pxr_pnp.cu": ["--fmad=false"]}
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++", "--expt-relaxed-constexpr",
@@ -29,7 +32,7 @@ def compile_one(name, verbose):
     obj = os.path.join(CSRC, name.replace(".cu", ".o"))
     if not _newer(src, obj):
         return name, "up to date"
-    cmd = [NVCC] + FLAGS + ["-c", src, "-o", obj]
+    cmd = [NVCC] + FLAGS + FILE_FLAGS.get(name, []) + ["-c", src, "-o", obj]
     r = subprocess.run(cmd, capture_output=True, text=True)
     log = os.path.join(CSRC, name.replace(".cu", ".ptxas.log"))
     with open(log, "w") as f:

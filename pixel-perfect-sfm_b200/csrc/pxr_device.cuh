@@ -262,6 +262,47 @@ __device__ __forceinline__ void cam_world_to_image(int model, const double* __re
   }
 }
 
+// (colmap 3.8 camera_models.h) ImageToWorld: pixel (x, y) -> normalised image point (u, v), the inverse of
+// cam_world_to_image.  The principal point and focal lengths are removed, then the distortion is undone by Newton steps
+// on the forward map (at most 100, until the squared step norm falls below 1e-28): COLMAP's IterativeUndistortion with
+// the analytic Jacobian Dm in place of central differences, so the inverse round-trips to the last bits.
+// OPENCV_FISHEYE solves its theta mapping theta_d = theta (1 + k1 theta^2 + ... + k4 theta^8) for theta instead.
+__device__ __forceinline__ void cam_image_to_world(int model, const double* __restrict__ p, double x, double y, double& u,
+                                                   double& v) {
+  const bool one_f = model == 0 || model == 2 || model == 3;
+  const double fx = p[0], fy = one_f ? p[0] : p[1];
+  const double cx = one_f ? p[1] : p[2], cy = one_f ? p[2] : p[3];
+  const double ud = (x - cx) / fx, vd = (y - cy) / fy;
+  u = ud; v = vd;
+  if (model == 0 || model == 1) return;
+  if (model == 5) {
+    const double thd = sqrt(ud * ud + vd * vd);
+    if (!(thd > 2.220446049250313e-16)) return;
+    double th = thd;
+    for (int it = 0; it < 100; ++it) {
+      const double t2 = th * th, t4 = t2 * t2, t6 = t4 * t2, t8 = t4 * t4;
+      const double f = th * (1.0 + p[4] * t2 + p[5] * t4 + p[6] * t6 + p[7] * t8) - thd;
+      const double fp = 1.0 + 3.0 * p[4] * t2 + 5.0 * p[5] * t4 + 7.0 * p[6] * t6 + 9.0 * p[7] * t8;
+      const double step = f / fp;
+      th -= step;
+      if (step * step < 1e-28) break;
+    }
+    const double s = tan(th) / thd;
+    u = ud * s; v = vd * s;
+    return;
+  }
+  double Jk[2][kMaxK], Dm[4];
+  for (int it = 0; it < 100; ++it) {
+    double px, py;
+    cam_world_to_image<true>(model, p, u, v, px, py, Dm, Jk);
+    const double rx = px - x, ry = py - y;
+    const double det = Dm[0] * Dm[3] - Dm[1] * Dm[2];
+    const double su = (Dm[3] * rx - Dm[1] * ry) / det, sv = (Dm[0] * ry - Dm[2] * rx) / det;
+    u -= su; v -= sv;
+    if (!(su * su + sv * sv >= 1e-28)) break;      // converged, or a NaN step
+  }
+}
+
 // WorldToPixel (projection.h:60-75) = ceres::QuaternionRotatePoint (normalising) + t, perspective
 // divide, camera model.  With JAC, returns d(xy)/d(local pose: 3 rot (QuaternionManifold
 // tangent, left-multiplicative) + 3 t), d(xy)/dX, d(xy)/d(cam params).

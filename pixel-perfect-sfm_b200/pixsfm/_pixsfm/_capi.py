@@ -188,6 +188,60 @@ class QKAResult(C.Structure):          # pxr_qka_result
                 ("final_cost", C.c_double), ("num_successful_steps", C.c_int32), ("num_unsuccessful_steps", C.c_int32),
                 ("num_iterations", C.c_int32), ("termination_type", C.c_int32)]
 
+class PnPDesc(C.Structure):            # pxr_pnp_desc
+    _fields_ = [("n_queries", C.c_int32), ("corr_begin", C.c_void_p), ("points2D", C.c_void_p), ("points3D", C.c_void_p),
+                ("cam_model", C.c_void_p), ("cam_params", C.c_void_p), ("seed", C.c_void_p), ("qvec", C.c_void_p),
+                ("tvec", C.c_void_p), ("inlier_mask", C.c_void_p)]
+
+
+class PnPOptions(C.Structure):         # pxr_pnp_options
+    _fields_ = [("max_error", C.c_double), ("min_inlier_ratio", C.c_double), ("min_num_trials", C.c_int32),
+                ("max_num_trials", C.c_int32), ("confidence", C.c_double), ("dyn_num_trials_multiplier", C.c_double),
+                ("estimate_focal_length", C.c_int32), ("refine", C.c_int32), ("gradient_tolerance", C.c_double),
+                ("max_num_iterations", C.c_int32), ("loss_function_scale", C.c_double), ("refine_focal_length", C.c_int32),
+                ("refine_extra_params", C.c_int32), ("function_tolerance", C.c_double), ("parameter_tolerance", C.c_double)]
+
+
+class PnPResult(C.Structure):          # pxr_pnp_result
+    _fields_ = [("status", C.c_int32), ("success", C.c_int32), ("num_inliers", C.c_int32), ("num_trials", C.c_int32),
+                ("best_trial", C.c_int32), ("best_solution", C.c_int32), ("local_optimized", C.c_int32),
+                ("num_iterations", C.c_int32), ("termination_type", C.c_int32), ("initial_cost", C.c_double),
+                ("final_cost", C.c_double)]
+
+
+def default_pnp_options(**kw):
+    o = PnPOptions()
+    load_lib().pxr_default_pnp_options(C.byref(o))
+    for k, v in kw.items():
+        if not hasattr(o, k):
+            raise ValueError("unknown pxr_pnp_options field '%s'" % k)
+        setattr(o, k, v)
+    return o
+
+
+class PnPBatch:
+    """numpy arrays of a batch of absolute pose estimations + the ctypes view (pxr_pnp_desc): per query camera model,
+    params [12] (in/out), seed, qvec / tvec (out); per correspondence a 2D point (pixels), a 3D point and the inlier flag
+    (out)."""
+
+    def __init__(self, corr_begin, points2D, points3D, cam_model, cam_params, seed):
+        self.corr_begin = _as(corr_begin, np.int64)
+        self.cam_model = _as(cam_model, np.int32)
+        nq = len(self.cam_model)
+        self.n_queries = nq
+        self.points2D = _as(points2D, np.float64, (-1, 2))
+        self.points3D = _as(points3D, np.float64, (-1, 3))
+        self.cam_params = _as(cam_params, np.float64, (nq, PXR_MAX_CAM_PARAMS))
+        self.seed = _as(seed, np.uint64)
+        self.qvec = np.zeros((nq, 4)); self.qvec[:, 0] = 1.0
+        self.tvec = np.zeros((nq, 3))
+        self.inlier_mask = np.zeros(len(self.points2D), np.uint8)
+
+    def desc(self):
+        return PnPDesc(self.n_queries, _ptr(self.corr_begin), _ptr(self.points2D), _ptr(self.points3D), _ptr(self.cam_model),
+                       _ptr(self.cam_params), _ptr(self.seed), _ptr(self.qvec), _ptr(self.tvec), _ptr(self.inlier_mask))
+
+
 class QBABatch:
     """numpy arrays of a batch of query bundle adjustments + the ctypes view (pxr_qba_desc).  Per query: camera model,
     params [12] (in/out), constancy mask, qvec / tvec (in/out), a patch block [n_q, H, W, C] (host numpy array or

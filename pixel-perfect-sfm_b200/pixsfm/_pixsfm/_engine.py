@@ -270,6 +270,47 @@ def qba_debug_linearize(batch, interp=None, options=None, ctx=None):
     return out
 
 
+def pnp_run(batch, options=None, ctx=None):
+    """pxr_pnp_run: absolute pose estimation for every query of a _capi.PnPBatch, one launch for the batch; writes qvec /
+    tvec (successful queries), cam_params (when refinement refines intrinsics) and inlier_mask into it.  -> (list of
+    per-query dicts with the pxr_pnp_result fields, dict(solve_time_s, total_time_s, kernel_launches, h2d_bytes))"""
+    ctx = ctx or _capi.default_context()
+    options = options or _capi.default_pnp_options()
+    d = batch.desc()
+    nq = batch.n_queries
+    res = (_capi.PnPResult * max(nq, 1))()
+    tot = _capi.make_summary(0)
+    _capi.check(ctx.lib.pxr_pnp_run(ctx.handle, C.byref(d), C.byref(options), res, C.byref(tot)))
+    out = [{f[0]: getattr(res[q], f[0]) for f in _capi.PnPResult._fields_} for q in range(nq)]
+    t = _capi.summary_to_dict(tot)
+    return out, dict(solve_time_s=t["solve_time_s"], total_time_s=t["total_time_s"], kernel_launches=t["kernel_launches"],
+                     h2d_bytes=t["h2d_bytes"])
+
+
+def pnp_debug_image_to_world(model, params, xy, ctx=None):
+    """pxr_pnp_debug_image_to_world: the device's ImageToWorld of pixels xy [n, 2] -> [n, 2]"""
+    ctx = ctx or _capi.default_context()
+    p = np.zeros(_capi.PXR_MAX_CAM_PARAMS)
+    p[:len(params)] = params
+    xy = np.ascontiguousarray(xy, np.float64).reshape(-1, 2)
+    out = np.zeros_like(xy)
+    _capi.check(ctx.lib.pxr_pnp_debug_image_to_world(ctx.handle, C.c_int32(int(model)), _p(p), C.c_int64(len(xy)), _p(xy),
+                                                     _p(out)))
+    return out
+
+
+def pnp_debug_p3p(x, X, ctx=None):
+    """pxr_pnp_debug_p3p: the device's P3P of triplets x [n, 3, 2] (normalised) and X [n, 3, 3] -> (poses [n, 4, 7]
+    (qvec with w >= 0 | tvec), n_sol [n])"""
+    ctx = ctx or _capi.default_context()
+    x = np.ascontiguousarray(x, np.float64).reshape(-1, 3, 2)
+    X = np.ascontiguousarray(X, np.float64).reshape(-1, 3, 3)
+    poses = np.zeros((len(x), 4, 7))
+    n_sol = np.zeros(len(x), np.int32)
+    _capi.check(ctx.lib.pxr_pnp_debug_p3p(ctx.handle, C.c_int64(len(x)), _p(x), _p(X), _p(poses), _p(n_sol)))
+    return poses, n_sol
+
+
 class PinnedArray:
     """A numpy array in pinned (page-locked, device-mapped) host memory from pxr_host_alloc_pinned: the patch source
     pxr_ba_run reads tap windows from directly (window residency, csrc/pxr_resident.cuh) and full-rate DMA otherwise.

@@ -492,3 +492,92 @@ class QueryBundleOptimizer:
     def summaries(self):
         """per-query summaries of the last run_batch (None for a query that was not solved)"""
         return getattr(self, "_summaries", [])
+
+
+# ---- absolute pose estimation (pycolmap 0.4 absolute_pose_estimation on pxr_pnp_run)
+# pycolmap 0.4's option names and defaults (AbsolutePoseEstimationOptions / RANSACOptions, AbsolutePoseRefinementOptions).
+# pycolmap is not a dependency of this package, so the defaults are restated from its 0.4 sources as best known and are
+# not checked against an installed copy.
+ABSOLUTE_POSE_ESTIMATION_DEFAULTS = dict(
+    estimate_focal_length=False, num_focal_length_samples=30, min_focal_length_ratio=0.2, max_focal_length_ratio=5.0,
+    ransac=dict(max_error=12.0, min_inlier_ratio=0.01, min_num_trials=1000, max_num_trials=100000, confidence=0.9999,
+                dyn_num_trials_multiplier=3.0))
+ABSOLUTE_POSE_REFINEMENT_DEFAULTS = dict(gradient_tolerance=1.0, max_num_iterations=100, loss_function_scale=1.0,
+                                         refine_focal_length=False, refine_extra_params=False, print_summary=False)
+
+
+def _merge_options(defaults, given, where):
+    out = {k: (dict(v) if isinstance(v, dict) else v) for k, v in defaults.items()}
+    for k, v in (given or {}).items():
+        if k not in defaults:
+            raise ValueError("%s: unknown option '%s'" % (where, k))
+        if isinstance(defaults[k], dict):
+            out[k] = _merge_options(defaults[k], v, where + "." + k)
+        else:
+            out[k] = v
+    return out
+
+
+def pnp_options(estimation_options=None, refinement_options=None):
+    """pycolmap-style nested option dicts (unknown keys rejected) merged over the defaults -> _capi.PnPOptions"""
+    est = _merge_options(ABSOLUTE_POSE_ESTIMATION_DEFAULTS, estimation_options, "estimation_options")
+    ref = _merge_options(ABSOLUTE_POSE_REFINEMENT_DEFAULTS, refinement_options, "refinement_options")
+    if est["estimate_focal_length"]:
+        raise ValueError("estimate_focal_length=True is not supported: the built-in absolute pose estimator estimates the "
+                         "pose only (refinement_options refine_focal_length refines the focal length after RANSAC)")
+    r = est["ransac"]
+    return _capi.default_pnp_options(
+        max_error=float(r["max_error"]), min_inlier_ratio=float(r["min_inlier_ratio"]),
+        min_num_trials=int(r["min_num_trials"]), max_num_trials=int(r["max_num_trials"]), confidence=float(r["confidence"]),
+        dyn_num_trials_multiplier=float(r["dyn_num_trials_multiplier"]), estimate_focal_length=0, refine=1,
+        gradient_tolerance=float(ref["gradient_tolerance"]), max_num_iterations=int(ref["max_num_iterations"]),
+        loss_function_scale=float(ref["loss_function_scale"]), refine_focal_length=int(bool(ref["refine_focal_length"])),
+        refine_extra_params=int(bool(ref["refine_extra_params"])))
+
+
+def absolute_pose_estimation_batch(queries, estimation_options=None, refinement_options=None, ctx=None):
+    """absolute_pose_estimation for every entry of `queries`, tuples (points2D [N,2], points3D [N,3], camera[, seed]), in
+    one pxr_pnp_run.  A query's result depends only on its own inputs and seed (default 0), never on the batch.  Returns
+    one pycolmap 0.4 dict per query: success, qvec, tvec, num_inliers, inliers (list of bool), or {"success": False}."""
+    opt = pnp_options(estimation_options, refinement_options)
+    queries = [tuple(q) for q in queries]
+    if not queries:
+        return []
+    p2, p3, begin, models, params, seeds = [], [], [0], [], [], []
+    for q in queries:
+        a2 = np.asarray(q[0], np.float64).reshape(-1, 2)
+        a3 = np.asarray([np.asarray(getattr(p, "xyz", p), np.float64) for p in q[1]], np.float64).reshape(-1, 3)
+        if len(a2) != len(a3):
+            raise ValueError("points2D and points3D must have the same length")
+        cam = q[2]
+        cp = np.zeros(_capi.PXR_MAX_CAM_PARAMS)
+        cp[:len(cam.params)] = np.asarray(cam.params, np.float64)
+        p2.append(a2); p3.append(a3); begin.append(begin[-1] + len(a2))
+        models.append(int(cam.model_id)); params.append(cp); seeds.append(int(q[3]) if len(q) > 3 else 0)
+    batch = _capi.PnPBatch(begin, np.concatenate(p2), np.concatenate(p3), models, params, np.array(seeds, np.uint64))
+    res, _ = _engine.pnp_run(batch, opt, ctx)
+    out = []
+    intrinsics = bool(opt.refine_focal_length or opt.refine_extra_params)
+    for k, (q, r) in enumerate(zip(queries, res)):
+        if not r["success"]:
+            out.append({"success": False})
+            continue
+        if intrinsics:
+            cam = q[2]
+            cam.params[:] = batch.cam_params[k, :len(cam.params)]
+        mask = batch.inlier_mask[begin[k]:begin[k + 1]]
+        out.append({"success": True, "qvec": batch.qvec[k].copy(), "tvec": batch.tvec[k].copy(),
+                    "num_inliers": int(r["num_inliers"]), "inliers": [bool(m) for m in mask]})
+    return out
+
+
+def absolute_pose_estimation(points2D, points3D, camera, estimation_options=None, refinement_options=None):
+    """pycolmap 0.4's absolute_pose_estimation on the device: LO-RANSAC over P3P (Lambda Twist) with the pixel threshold
+    estimation_options["ransac"]["max_error"], then a Cauchy-robust refinement of the pose over the inliers (and of the
+    focal length / extra parameters when refinement_options ask: camera.params is then updated in place).  Options use
+    pycolmap's nested names; unknown keys raise.  Defaults (pycolmap 0.4 as best known, unverified against an installed
+    pycolmap): ransac max_error 12, min_inlier_ratio 0.01, min_num_trials 1000, max_num_trials 100000, confidence
+    0.9999, dyn_num_trials_multiplier 3; refinement gradient_tolerance 1, max_num_iterations 100, loss_function_scale 1,
+    refine_focal_length / refine_extra_params False.  Returns dict(success, qvec, tvec, num_inliers, inliers) or
+    {"success": False}; estimate_focal_length=True is not supported."""
+    return absolute_pose_estimation_batch([(points2D, points3D, camera)], estimation_options, refinement_options)[0]

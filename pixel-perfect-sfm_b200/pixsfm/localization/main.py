@@ -1,6 +1,8 @@
 """pixsfm.localization.main — the reference's query refinement surface (pixsfm/localization/main.py:20-330): helper
-functions, QueryKeypointAdjuster, QueryBundleAdjuster and a QueryLocalizer whose PnP step is pluggable (the reference
-calls pycolmap.absolute_pose_estimation, which is not part of this package)."""
+functions, QueryKeypointAdjuster, QueryBundleAdjuster and a QueryLocalizer whose PnP step is pluggable: a given
+callable, else pycolmap.absolute_pose_estimation (the reference's call) when pycolmap imports, else the built-in
+absolute_pose_estimation (LO-RANSAC over P3P and a robust pose refinement on the GPU, batched over the queries of
+localize_batch)."""
 import numpy as np
 
 from .. import defaults
@@ -207,9 +209,10 @@ class QueryLocalizer:
     """QKA -> PnP -> QBA for one query image (reference localization/main.py:262-537), with the reference's constructor
     and `localize` signatures.  Holds the reconstruction and one {point3D_id: Reference} map per feature level: given
     (`references=`), or extracted at construction from `dense_features` (a FeatureManager, or the path of a feature cache)
-    or from features the `extractor` computes for `image_dir`.  The absolute-pose step is pycolmap.absolute_pose_estimation
-    when pycolmap imports; `pose_estimator(points2D [N,2], points3D [N,3], camera) -> dict(success, qvec, tvec, inliers)`
-    replaces it (pycolmap is outside this package)."""
+    or from features the `extractor` computes for `image_dir`.  The absolute-pose step is `pose_estimator(points2D [N,2],
+    points3D [N,3], camera) -> dict(success, qvec, tvec, inliers)` when one is given, else
+    pycolmap.absolute_pose_estimation when pycolmap imports, else this package's absolute_pose_estimation (the conf's
+    PnP.estimation / PnP.refinement merged over its pycolmap defaults)."""
     default_conf = defaults.query_localizer()
 
     def __init__(self, reconstruction, conf=None, dense_features=None, image_dir=None, references=None, extractor=None,
@@ -292,17 +295,27 @@ class QueryLocalizer:
         manager = self.extractor.features_from_image_list(None, [name], {name: keypoints}, {name: required_kp_ids})
         return [manager.fset(level).fmap(name) for level in range(manager.num_levels)]
 
-    def _absolute_pose(self, pnp_points2D, pnp_points3D, query_camera, pose_estimator):
+    def _pose_estimator(self, pose_estimator=None):
+        """the per-query PnP callable: `pose_estimator`, else the localizer's, else pycolmap.absolute_pose_estimation when
+        pycolmap imports; None: the built-in estimator (absolute_pose_estimation on the device), batched over queries"""
         estimator = pose_estimator or self.pose_estimator
         if estimator is not None:
-            return estimator(pnp_points2D, np.array(pnp_points3D), query_camera)
+            return lambda p2D, p3D, camera: estimator(p2D, np.array(p3D), camera)
         try:
             import pycolmap
         except ImportError:
-            raise ValueError("a pose_estimator callable is required (pycolmap.absolute_pose_estimation is not importable)")
-        return pycolmap.absolute_pose_estimation(pnp_points2D, pnp_points3D, query_camera,
-                                                 estimation_options=to_ctr(self.conf.PnP.estimation),
-                                                 refinement_options=to_ctr(self.conf.PnP.refinement))
+            return None
+        return lambda p2D, p3D, camera: pycolmap.absolute_pose_estimation(
+            p2D, p3D, camera, estimation_options=to_ctr(self.conf.PnP.estimation),
+            refinement_options=to_ctr(self.conf.PnP.refinement))
+
+    def _absolute_pose(self, pnp_points2D, pnp_points3D, query_camera, pose_estimator):
+        estimator = self._pose_estimator(pose_estimator)
+        if estimator is not None:
+            return estimator(pnp_points2D, pnp_points3D, query_camera)
+        return loc.absolute_pose_estimation(pnp_points2D, pnp_points3D, query_camera,
+                                            estimation_options=to_ctr(self.conf.PnP.estimation),
+                                            refinement_options=to_ctr(self.conf.PnP.refinement))
 
     def localize(self, keypoints, pnp_point2D_idxs, pnp_points3D_id, query_camera, image_path=None, query_fmaps=None,
                  pose_estimator=None):
@@ -321,8 +334,8 @@ class QueryLocalizer:
     def localize_batch(self, queries, max_wave_bytes=0.0):
         """localize() for every entry of `queries` (dicts of localize's keyword arguments): per feature level the
         reference selection of every query at once (one pxr_query_match_run for target_reference 'nearest', against the
-        level's stored observations packed once and kept in device memory), per level one batched QKA solve, PnP per
-        query, one batched QBA solve per level over every query that has a pose, then the per-query inlier
+        level's stored observations packed once and kept in device memory), per level one batched QKA solve, PnP (one
+        pxr_pnp_run for every query on the built-in estimator, else per query), one batched QBA solve per level over every query that has a pose, then the per-query inlier
         recomputation.  Returns the list of pose dicts localize would return."""
         states = [self._localize_prepare(**q) for q in queries]
         live = [st for st in states if "result" not in st]
@@ -344,7 +357,14 @@ class QueryLocalizer:
             if self.conf.QKA.apply:
                 self.query_keypoint_adjuster.refine_multilevel_batch(
                     [(st["points2D"], st["fmaps"], st["references"], st["point2D_idxs"]) for st in live], max_wave_bytes)
-        states = [st if "result" in st else self._localize_pose(st) for st in states]
+        builtin = [st for st in states if "result" not in st and self._pose_estimator(st["pose_estimator"]) is None]
+        poses = {}
+        if builtin:                                           # the built-in estimator: every such query in one launch
+            found = loc.absolute_pose_estimation_batch([(st["points2D"], st["points3D"], st["camera"]) for st in builtin],
+                                                       estimation_options=to_ctr(self.conf.PnP.estimation),
+                                                       refinement_options=to_ctr(self.conf.PnP.refinement))
+            poses = {id(st): pose for st, pose in zip(builtin, found)}
+        states = [st if "result" in st else self._localize_pose(st, poses.get(id(st))) for st in states]
         live = [st for st in states if "result" not in st]
         if self.conf.QBA.apply and live:
             self.query_bundle_adjuster.refine_multilevel_batch([self._qba_args(st) for st in live], max_wave_bytes)
@@ -403,10 +423,12 @@ class QueryLocalizer:
                 "fmaps": query_fmaps, "references": None, "point2D_idxs": pnp_point2D_idxs, "require_feats": require_feats,
                 "pose_estimator": pose_estimator}
 
-    def _localize_pose(self, st):
-        """PnP on the (refined) correspondences and the inlier selection: {"result": pose dict} when PnP fails"""
+    def _localize_pose(self, st, pose_dict=None):
+        """PnP on the (refined) correspondences (unless its pose dict is given) and the inlier selection: {"result": pose
+        dict} when PnP fails"""
         pnp_points2D, pnp_points3D, query_camera = st["points2D"], st["points3D"], st["camera"]
-        pose_dict = self._absolute_pose(pnp_points2D, pnp_points3D, query_camera, st["pose_estimator"])
+        if pose_dict is None:
+            pose_dict = self._absolute_pose(pnp_points2D, pnp_points3D, query_camera, st["pose_estimator"])
         if not pose_dict.get("success", False):
             return {"result": pose_dict}
         inliers = pose_dict.get("inliers", [True] * len(pnp_points3D))
