@@ -738,6 +738,73 @@ int pxr_pnp_debug_image_to_world(pxr_ctx* ctx, int32_t model, const double* para
                                  double* out);
 int pxr_pnp_debug_p3p(pxr_ctx* ctx, int64_t n, const double* x, const double* X, double* poses, int32_t* n_sol);
 
+/* ---- point triangulation from known poses ------------------------------------------
+ * COLMAP's point_triangulator as hloc's triangulation drives it, with poses and intrinsics fixed (csrc/pxr_tri.cu).
+ *  pxr_tri_verify  geometric verification of matches (hloc's geometric_verification): both keypoints go to the
+ *                  normalised plane (ImageToWorld), E = [t]x R of cam1_from_cam0, and the two point-to-epipolar-line
+ *                  distances d0 = |x1^T E x0| / |(E^T x1)_{0,1}|, d1 = |x1^T E x0| / |(E x0)_{0,1}|; a match is kept when
+ *                  d_k <= noise_k * max_error / mean focal length of camera k (COLMAP's CamFromImgThreshold).
+ *  pxr_tri_run     robust triangulation of every track, one warp per track.  Each observation becomes a world ray
+ *                  (unit direction d, camera centre c).  Hypotheses are observation pairs: all n(n-1)/2 of them in
+ *                  lexicographic order when that is <= tri_max_pairs, else tri_max_pairs sampled ones, hypothesis h
+ *                  drawing words w_k = splitmix64(s0 ^ (h << 8) ^ k), k = 0, 1, ... 63, s0 = splitmix64(seed ^
+ *                  splitmix64(key)), key = track_key[t] (or t when NULL), taking index ((w_k >> 32) * n) >> 32 from each
+ *                  and keeping the first two distinct ones (none after 64 draws: no hypothesis).  A pair whose rays are
+ *                  less than min_angle apart makes no hypothesis.  Its point is the midpoint least-squares point
+ *                  X = (sum (I - d d^T))^-1 sum (I - d d^T) c.  The error of an observation is the angle between d and
+ *                  X - c, in [0, 180]; an inlier has (X - c).d > 0 (in front of the camera along its ray) and error <=
+ *                  create_max_angle_error; an observation that is not in front scores as one at the threshold.  Score: MSAC sum min(e^2, tau^2); the lowest score wins, ties to the lowest
+ *                  hypothesis index.  The winner's inliers S0 give X1 = midpoint(S0); when the inliers S1 of X1 differ
+ *                  from S0, X2 = midpoint(S1).  The result is the last point and the set it was fitted to.
+ *  pxr_tri_evaluate  the per-observation pixel errors and per-track angles of given points, no RANSAC.
+ * Angles are in degrees.  The triangulation angle of a point is COLMAP's CalculateTriangulationAngle: the angle at X
+ * between X - c_i and X - c_j, folded to min(a, 180 - a), largest over the pairs of the set (inliers in run mode, every
+ * observation in evaluate mode). */
+typedef struct {
+  int32_t n_cameras;
+  const int32_t* cam_model;       /* [n_cameras] pxr_camera_model */
+  const double* cam_params;       /* [n_cameras][PXR_MAX_CAM_PARAMS] */
+  int32_t n_images;
+  const int32_t* img_cam;         /* [n_images] camera index */
+  const double* qvec;             /* [n_images][4] (w,x,y,z) world->camera */
+  const double* tvec;             /* [n_images][3] */
+  int64_t n_tracks;
+  const int64_t* track_begin;     /* [n_tracks+1] from 0, >= 2 observations per track */
+  const int64_t* track_key;       /* [n_tracks] sample-stream key, or NULL (the track index) */
+  const int32_t* obs_img;         /* [n_obs] image index */
+  const double* obs_xy;           /* [n_obs][2] pixels, COLMAP convention */
+} pxr_tri_desc;
+
+typedef struct {
+  double min_angle;               /* degrees: hypothesis pairs and points below it are rejected */
+  double create_max_angle_error;  /* degrees: inlier threshold of the angular error */
+  int32_t tri_max_pairs;          /* hypotheses of a track at most (exhaustive up to this many pairs) */
+  uint64_t seed;
+} pxr_tri_options;
+
+enum { PXR_TRI_OK = 0, PXR_TRI_TOO_FEW_INLIERS = 1, PXR_TRI_ANGLE_TOO_SMALL = 2 };
+
+/* min_angle 1.5, create_max_angle_error 2 (COLMAP's IncrementalTriangulator), tri_max_pairs 1024, seed 0 */
+void pxr_default_tri_options(pxr_tri_options* opt);
+/* Verifies n_matches matches in one launch (tracks in desc are not read).  match_img [n][2] image indices,
+ * match_xy [n][4] (x0, y0, x1, y1) pixels, match_noise [n][2] keypoint noise (pixels) of each side; keep [n] and
+ * err [n][2] (normalised-plane distances d0, d1) out. */
+int pxr_tri_verify(pxr_ctx* ctx, const pxr_tri_desc* desc, int64_t n_matches, const int32_t* match_img,
+                   const double* match_xy, const double* match_noise, double max_error, uint8_t* keep, double* err,
+                   pxr_summary* total);
+/* Triangulates every track.  Out: xyz [n_tracks][3], status [n_tracks] (PXR_TRI_*), n_inliers [n_tracks],
+ * tri_angle [n_tracks] (of the inliers), obs_inlier [n_obs], obs_error [n_obs] pixel reprojection error of the
+ * returned point (+inf behind the camera).  A track's results depend only on its own observations, key and seed. */
+int pxr_tri_run(pxr_ctx* ctx, const pxr_tri_desc* desc, const pxr_tri_options* opt, double* xyz, int32_t* status,
+                int32_t* n_inliers, double* tri_angle, uint8_t* obs_inlier, double* obs_error, pxr_summary* total);
+/* obs_error [n_obs] and tri_angle [n_tracks] (every observation) of the points xyz [n_tracks][3]. */
+int pxr_tri_evaluate(pxr_ctx* ctx, const pxr_tri_desc* desc, const double* xyz, double* obs_error, double* tri_angle,
+                     pxr_summary* total);
+/* total (or NULL): solve_time_s = device time of the kernels (CUDA events), total_time_s, kernel launches, h2d_bytes.
+ * All three check their arguments before the context: NULL arrays, negative counts, an unknown camera model, an index
+ * out of range, a track_begin that does not start at 0 or is not increasing by >= 2, bad options:
+ * PXR_ERR_INVALID_ARGUMENT / PXR_ERR_UNSUPPORTED without a device. */
+
 /* ---- batched query keypoint adjustment ------------------------------------------
  * replaces a loop of _localization.QueryKeypointOptimizer.run: N independent queries, each one problem of pxr_ka_run's
  * query mode (every residual block = one keypoint against one fixed descriptor).  One CTA solves one query; the

@@ -447,6 +447,72 @@ PYBIND11_MODULE(_pxr_pybind, m) {
     }
     return py::dict("results"_a = out, "solve_time_s"_a = s.solve_time_s, "total_time_s"_a = s.total_time_s);
   }, "ctx"_a, "problem"_a, "options"_a = py::dict());
+  // triangulation from known poses: `problem` holds cam_model [nc], cam_params [nc,12], img_cam [ni], qvec [ni,4],
+  // tvec [ni,3] and, for tri_run, track_begin [nt+1], obs_img [n], obs_xy [n,2] and optionally track_key [nt]
+  auto tri_desc = [](Fields& f, bool tracks) {
+    pxr_tri_desc d;
+    std::memset(&d, 0, sizeof(d));
+    d.n_cameras = (int32_t)f.len("cam_model");
+    d.cam_model = f.arr<int32_t>("cam_model");
+    d.cam_params = f.arr<double>("cam_params");
+    d.n_images = (int32_t)f.len("img_cam");
+    d.img_cam = f.arr<int32_t>("img_cam");
+    d.qvec = f.arr<double>("qvec");
+    d.tvec = f.arr<double>("tvec");
+    if (tracks) {
+      d.track_begin = f.arr<int64_t>("track_begin");
+      d.n_tracks = f.len("track_begin") - 1;
+      if (d.n_tracks < 0) throw py::value_error("track_begin must hold n_tracks + 1 entries");
+      d.track_key = f.arr<int64_t>("track_key", false);
+      if (d.track_key && f.len("track_key") != d.n_tracks) throw py::value_error("track_key must hold n_tracks entries");
+      d.obs_img = f.arr<int32_t>("obs_img", false);
+      d.obs_xy = f.arr<double>("obs_xy", false);
+      if (f.len("obs_img") != d.track_begin[d.n_tracks] || f.len("obs_xy") != d.track_begin[d.n_tracks])
+        throw py::value_error("obs_img / obs_xy must hold track_begin[-1] entries");
+    }
+    return d;
+  };
+  m.def("tri_verify", [tri_desc](Context& ctx, py::dict problem, carray<int32_t> match_img, carray<double> match_xy,
+                                 carray<double> match_noise, double max_error) {
+    Fields f{problem, {}};
+    const pxr_tri_desc d = tri_desc(f, false);
+    const int64_t n = match_img.size() / 2;
+    if (match_img.size() != 2 * n || match_xy.size() != 4 * n || match_noise.size() != 2 * n)
+      throw py::value_error("match_img [n,2], match_xy [n,4] and match_noise [n,2] differ in n");
+    carray<uint8_t> keep(n);
+    carray<double> err({n, (int64_t)2});
+    int rc;
+    { py::gil_scoped_release nogil;
+      rc = pxr_tri_verify(ctx.h, &d, n, match_img.data(), match_xy.data(), match_noise.data(), max_error,
+                          keep.mutable_data(), err.mutable_data(), nullptr); }
+    check(rc);
+    return py::dict("keep"_a = keep, "err"_a = err);
+  }, "ctx"_a, "problem"_a, "match_img"_a, "match_xy"_a, "match_noise"_a, "max_error"_a = 4.0);
+  m.def("tri_run", [tri_desc](Context& ctx, py::dict problem, py::dict options) {
+    Fields f{problem, {}};
+    const pxr_tri_desc d = tri_desc(f, true);
+    pxr_tri_options o; pxr_default_tri_options(&o);
+    for (auto item : options) {
+      const std::string k = py::str(item.first);
+      py::handle v = item.second;
+      if (k == "min_angle") o.min_angle = v.cast<double>();
+      else if (k == "create_max_angle_error") o.create_max_angle_error = v.cast<double>();
+      else if (k == "tri_max_pairs") o.tri_max_pairs = v.cast<int32_t>();
+      else if (k == "seed") o.seed = v.cast<uint64_t>();
+      else throw py::value_error("unknown triangulation option '" + k + "'");
+    }
+    const int64_t nt = d.n_tracks, no = d.track_begin[nt];
+    carray<double> xyz({nt, (int64_t)3}), angle(nt), err(no);
+    carray<int32_t> status(nt), n_inl(nt);
+    carray<uint8_t> inl(no);
+    int rc;
+    { py::gil_scoped_release nogil;
+      rc = pxr_tri_run(ctx.h, &d, &o, xyz.mutable_data(), status.mutable_data(), n_inl.mutable_data(), angle.mutable_data(),
+                       inl.mutable_data(), err.mutable_data(), nullptr); }
+    check(rc);
+    return py::dict("xyz"_a = xyz, "status"_a = status, "n_inliers"_a = n_inl, "tri_angle"_a = angle,
+                    "obs_inlier"_a = inl, "obs_error"_a = err);
+  }, "ctx"_a, "problem"_a, "options"_a = py::dict());
   // batched query KA (a loop of QueryKeypointOptimizer.run): per query kp_begin [nq+1], patches_are_sparse [nq] and
   // one host patch block (`patch_blocks`, `corner` / `scale` back to back); per keypoint keypoints [n,2] (refined IN
   // PLACE), kp_patch (within its query's block) and desc_begin [n+1] into descs [m, C]

@@ -134,6 +134,29 @@ __host__ __device__ __forceinline__ int cam_num_params(int model) {
 
 constexpr int kMaxK = 12;  // PXR_MAX_CAM_PARAMS
 
+// the mean of a model's focal lengths (COLMAP's MeanFocalLength): pixel thresholds over it are normalised-plane ones
+__device__ __forceinline__ double mean_focal(int model, const double* p) {
+  return (model == 0 || model == 2 || model == 3) ? p[0] : 0.5 * (p[0] + p[1]);
+}
+
+// normalised unit quaternion (w, x, y, z) -> rotation matrix (row-major)
+__device__ __forceinline__ void quat_to_rot(const double* qv, double* R) {
+  const double s = 1.0 / sqrt(qv[0] * qv[0] + qv[1] * qv[1] + qv[2] * qv[2] + qv[3] * qv[3]);
+  const double w = qv[0] * s, a = qv[1] * s, b = qv[2] * s, c = qv[3] * s;
+  R[0] = 1.0 - 2.0 * (b * b + c * c); R[1] = 2.0 * (a * b - w * c); R[2] = 2.0 * (a * c + w * b);
+  R[3] = 2.0 * (a * b + w * c); R[4] = 1.0 - 2.0 * (a * a + c * c); R[5] = 2.0 * (b * c - w * a);
+  R[6] = 2.0 * (a * c - w * b); R[7] = 2.0 * (b * c + w * a); R[8] = 1.0 - 2.0 * (a * a + b * b);
+}
+
+// the counter-based stream of the RANSAC samplers (include/pxr.h states it); integer code, so every translation unit
+// draws the same words whatever its floating-point flags
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
+  uint64_t z = x + 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
 // (colmap 3.8 camera_models.h) WorldToImage + derivatives.
 // Dm = d(x,y)/d(u,v) row-major 2x2; Jk[0][k] = dx/dp_k, Jk[1][k] = dy/dp_k.
 template <bool JAC>

@@ -35,13 +35,6 @@ constexpr int kCorrBytes = 40;                       // u, v, X, Y, Z
 constexpr size_t kPCorrSmem = 96 * 1024;             // a query's correspondences stay on chip up to 2457 of them
 constexpr double kDblEps = 2.220446049250313e-16;
 
-__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-  uint64_t z = x + 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
 // the three indices trial t draws (include/pxr.h); false when 64 draws give fewer than three distinct ones
 __device__ __forceinline__ bool draw_sample(uint64_t s0, int64_t t, int64_t n, int idx[3]) {
   int k = 0;
@@ -263,15 +256,6 @@ static __device__ void rot_to_quat(const double* R, double* q) {
   for (int k = 0; k < 4; ++k) q[k] = sg * (q[k] / n);
 }
 
-// normalised unit quaternion -> rotation matrix (row-major)
-static __device__ void quat_to_rot(const double* qv, double* R) {
-  const double s = 1.0 / sqrt(qv[0] * qv[0] + qv[1] * qv[1] + qv[2] * qv[2] + qv[3] * qv[3]);
-  const double w = qv[0] * s, a = qv[1] * s, b = qv[2] * s, c = qv[3] * s;
-  R[0] = 1.0 - 2.0 * (b * b + c * c); R[1] = 2.0 * (a * b - w * c); R[2] = 2.0 * (a * c + w * b);
-  R[3] = 2.0 * (a * b + w * c); R[4] = 1.0 - 2.0 * (a * a + c * c); R[5] = 2.0 * (b * c - w * a);
-  R[6] = 2.0 * (a * c - w * b); R[7] = 2.0 * (b * c + w * a); R[8] = 1.0 - 2.0 * (a * a + b * b);
-}
-
 // the squared normalised-plane error of one correspondence; false when the point is not in front of the camera
 __device__ __forceinline__ bool pnp_residual(const double* P, double u, double v, double X, double Y, double Z, double& r) {
   const double x = P[0] * X + P[1] * Y + P[2] * Z + P[9];
@@ -281,10 +265,6 @@ __device__ __forceinline__ bool pnp_residual(const double* P, double u, double v
   const double du = x * iz - u, dv = y * iz - v;
   r = du * du + dv * dv;
   return z > kDblEps;
-}
-
-__device__ __forceinline__ double mean_focal(int model, const double* p) {
-  return (model == 0 || model == 2 || model == 3) ? p[0] : 0.5 * (p[0] + p[1]);
 }
 
 struct Support { int cnt; double sum; int idx; };

@@ -242,6 +242,58 @@ class PnPBatch:
                        _ptr(self.cam_params), _ptr(self.seed), _ptr(self.qvec), _ptr(self.tvec), _ptr(self.inlier_mask))
 
 
+class TriDesc(C.Structure):            # pxr_tri_desc
+    _fields_ = [("n_cameras", C.c_int32), ("cam_model", C.c_void_p), ("cam_params", C.c_void_p), ("n_images", C.c_int32),
+                ("img_cam", C.c_void_p), ("qvec", C.c_void_p), ("tvec", C.c_void_p), ("n_tracks", C.c_int64),
+                ("track_begin", C.c_void_p), ("track_key", C.c_void_p), ("obs_img", C.c_void_p), ("obs_xy", C.c_void_p)]
+
+
+class TriOptions(C.Structure):         # pxr_tri_options
+    _fields_ = [("min_angle", C.c_double), ("create_max_angle_error", C.c_double), ("tri_max_pairs", C.c_int32),
+                ("seed", C.c_uint64)]
+
+
+# pxr_tri_run's per-track status
+TRI_OK, TRI_TOO_FEW_INLIERS, TRI_ANGLE_TOO_SMALL = range(3)
+
+
+def default_tri_options(**kw):
+    o = TriOptions()
+    load_lib().pxr_default_tri_options(C.byref(o))
+    for k, v in kw.items():
+        if not hasattr(o, k):
+            raise ValueError("unknown pxr_tri_options field '%s'" % k)
+        setattr(o, k, v)
+    return o
+
+
+class TriScene:
+    """numpy arrays of a triangulation problem + the ctypes view (pxr_tri_desc): cameras (model, params [12]), images
+    (camera index, qvec, tvec) and, for pxr_tri_run / pxr_tri_evaluate, tracks in CSR form (track_begin, per observation
+    the image index and the pixel)."""
+
+    def __init__(self, cam_model, cam_params, img_cam, qvec, tvec, track_begin=None, obs_img=None, obs_xy=None,
+                 track_key=None):
+        self.cam_model = _as(cam_model, np.int32)
+        self.cam_params = _as(cam_params, np.float64, (len(self.cam_model), PXR_MAX_CAM_PARAMS))
+        self.img_cam = _as(img_cam, np.int32)
+        self.qvec = _as(qvec, np.float64, (-1, 4))
+        self.tvec = _as(tvec, np.float64, (-1, 3))
+        self.track_begin = _as(track_begin if track_begin is not None else [0], np.int64)
+        self.obs_img = _as(obs_img if obs_img is not None else [], np.int32)
+        self.obs_xy = _as(obs_xy if obs_xy is not None else np.zeros((0, 2)), np.float64, (-1, 2))
+        self.track_key = None if track_key is None else _as(track_key, np.int64)
+
+    @property
+    def n_tracks(self):
+        return len(self.track_begin) - 1
+
+    def desc(self):
+        return TriDesc(len(self.cam_model), _ptr(self.cam_model), _ptr(self.cam_params), len(self.img_cam), _ptr(self.img_cam),
+                       _ptr(self.qvec), _ptr(self.tvec), self.n_tracks, _ptr(self.track_begin), _ptr(self.track_key),
+                       _ptr(self.obs_img), _ptr(self.obs_xy))
+
+
 class QBABatch:
     """numpy arrays of a batch of query bundle adjustments + the ctypes view (pxr_qba_desc).  Per query: camera model,
     params [12] (in/out), constancy mask, qvec / tvec (in/out), a patch block [n_q, H, W, C] (host numpy array or

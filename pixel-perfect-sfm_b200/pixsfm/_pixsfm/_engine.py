@@ -311,6 +311,63 @@ def pnp_debug_p3p(x, X, ctx=None):
     return poses, n_sol
 
 
+def _timing(tot):
+    t = _capi.summary_to_dict(tot)
+    return dict(solve_time_s=t["solve_time_s"], total_time_s=t["total_time_s"], kernel_launches=t["kernel_launches"],
+                h2d_bytes=t["h2d_bytes"])
+
+
+def tri_verify(scene, match_img, match_xy, match_noise, max_error=4.0, ctx=None):
+    """pxr_tri_verify: geometric verification of matches against the known poses of a _capi.TriScene.  match_img [n, 2]
+    image indices, match_xy [n, 4] pixels (x0, y0, x1, y1), match_noise [n, 2] -> (keep bool [n], err [n, 2] epipolar
+    distances in the normalised plane, timing dict)"""
+    ctx = ctx or _capi.default_context()
+    mi = np.ascontiguousarray(match_img, np.int32).reshape(-1, 2)
+    mx = np.ascontiguousarray(match_xy, np.float64).reshape(-1, 4)
+    mn = np.ascontiguousarray(match_noise, np.float64).reshape(-1, 2)
+    if not (len(mi) == len(mx) == len(mn)):
+        raise ValueError("match_img, match_xy and match_noise differ in length")
+    keep = np.zeros(len(mi), np.uint8)
+    err = np.zeros((len(mi), 2))
+    d = scene.desc()
+    tot = _capi.make_summary(0)
+    _capi.check(ctx.lib.pxr_tri_verify(ctx.handle, C.byref(d), C.c_int64(len(mi)), _p(mi), _p(mx), _p(mn),
+                                       C.c_double(max_error), _p(keep), _p(err), C.byref(tot)))
+    return keep.astype(bool), err, _timing(tot)
+
+
+def tri_run(scene, options=None, ctx=None):
+    """pxr_tri_run: robust triangulation of every track of a _capi.TriScene -> dict(xyz [nt, 3], status [nt] (TRI_*),
+    n_inliers [nt], tri_angle [nt] degrees, obs_inlier bool [n_obs], obs_error [n_obs] pixels, timing)"""
+    ctx = ctx or _capi.default_context()
+    options = options or _capi.default_tri_options()
+    nt, no = scene.n_tracks, int(scene.track_begin[-1])
+    out = dict(xyz=np.zeros((nt, 3)), status=np.zeros(nt, np.int32), n_inliers=np.zeros(nt, np.int32),
+               tri_angle=np.zeros(nt), obs_inlier=np.zeros(no, np.uint8), obs_error=np.zeros(no))
+    d = scene.desc()
+    tot = _capi.make_summary(0)
+    _capi.check(ctx.lib.pxr_tri_run(ctx.handle, C.byref(d), C.byref(options), _p(out["xyz"]), _p(out["status"]),
+                                    _p(out["n_inliers"]), _p(out["tri_angle"]), _p(out["obs_inlier"]), _p(out["obs_error"]),
+                                    C.byref(tot)))
+    out["obs_inlier"] = out["obs_inlier"].astype(bool)
+    out["timing"] = _timing(tot)
+    return out
+
+
+def tri_evaluate(scene, xyz, ctx=None):
+    """pxr_tri_evaluate: pixel reprojection errors [n_obs] (+inf behind the camera) and triangulation angles [nt]
+    (degrees, every observation) of the points xyz [nt, 3] -> (obs_error, tri_angle, timing)"""
+    ctx = ctx or _capi.default_context()
+    xyz = np.ascontiguousarray(xyz, np.float64).reshape(-1, 3)
+    if len(xyz) != scene.n_tracks:
+        raise ValueError("xyz must hold one point per track")
+    err, ang = np.zeros(int(scene.track_begin[-1])), np.zeros(scene.n_tracks)
+    d = scene.desc()
+    tot = _capi.make_summary(0)
+    _capi.check(ctx.lib.pxr_tri_evaluate(ctx.handle, C.byref(d), _p(xyz), _p(err), _p(ang), C.byref(tot)))
+    return err, ang, _timing(tot)
+
+
 class PinnedArray:
     """A numpy array in pinned (page-locked, device-mapped) host memory from pxr_host_alloc_pinned: the patch source
     pxr_ba_run reads tap windows from directly (window residency, csrc/pxr_resident.cuh) and full-rate DMA otherwise.

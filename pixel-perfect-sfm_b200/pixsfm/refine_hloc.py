@@ -7,8 +7,9 @@ or triangulator, which the reference reaches through `hloc.reconstruction.main` 
 (refine_hloc.py:100-115) — is not part of the featuremetric path: it is called through `sfm_backend`, an object with
 those two `main`-style callables (`reconstruction(model_path, image_dir, pairs_path, keypoints_path, matches_path, **args)`,
 `triangulation(model_path, reference_model_path, image_dir, pairs_path, keypoints_path, matches_path, **args)`), which
-defaults to hloc when it can be imported.  Without either the method raises, like the reference does ("Could not import
-hloc.")."""
+defaults to hloc when it can be imported.  Without hloc, triangulation against a reference model runs on this package's
+own triangulator (pixsfm.triangulation.main, same arguments); incremental mapping still raises, like the reference does
+("Could not import hloc.")."""
 from pathlib import Path
 
 from . import logger
@@ -88,11 +89,15 @@ class PixSfM(PixSfM_colmap):
 
     def run_reconstruction(self, output_dir, image_dir, pairs_path, keypoints_path, matches_path, reference_model_path=None,
                            **hloc_args):
-        if self.sfm_backend is None:
+        if self.sfm_backend is None and reference_model_path is None:
             raise ValueError("Could not import hloc.")
         model_path = Path(output_dir) / "hloc"
         model_path.mkdir(exist_ok=True, parents=False)
-        if reference_model_path is None:
+        if self.sfm_backend is None:
+            # without hloc, triangulation against the reference model runs on this package's own triangulator
+            from .triangulation import main as triangulate
+            triangulate(model_path, reference_model_path, image_dir, pairs_path, keypoints_path, matches_path, **hloc_args)
+        elif reference_model_path is None:
             self.sfm_backend.reconstruction(model_path, image_dir, pairs_path, keypoints_path, matches_path, **hloc_args)
         else:
             self.sfm_backend.triangulation(model_path, reference_model_path, image_dir, pairs_path, keypoints_path,

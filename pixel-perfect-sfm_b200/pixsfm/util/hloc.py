@@ -64,6 +64,18 @@ def read_keypoints_hloc(path, names=None, as_cpp_map=False):
         return {name: np.asarray(f[name]["keypoints"])[:, :2].astype(np.float64) for name in names}
 
 
+def read_keypoint_uncertainty(path, names):
+    """{name: the `uncertainty` attribute of the image's keypoint dataset, or None}: the keypoint noise in pixels that
+    hloc's feature extraction records (hloc.utils.io.get_keypoints(..., return_uncertainty=True))"""
+    h5py = _h5py()
+    with h5py.File(str(path), "r") as f:
+        out = {}
+        for name in names:
+            u = f[name]["keypoints"].attrs.get("uncertainty")
+            out[name] = None if u is None else float(np.asarray(u).reshape(-1)[0])
+        return out
+
+
 def write_keypoints_hloc(path, keypoint_dict):
     h5py = _h5py()
     with h5py.File(str(path), "w") as f:
