@@ -532,6 +532,33 @@ int pxr_dsift(pxr_ctx* ctx, const uint8_t* image, int32_t image_on_device, int32
               int32_t l2_normalize, const int32_t* corners, int64_t n_patches, int32_t patch_size, int32_t out_dtype,
               void* out_host, void** out_device);
 
+/* ---- S2DNet -> patch slab -------------------------------------------------
+ * replaces the reference's `s2dnet` model with num_layers 1 (features/models/s2dnet.py: VGG16's conv1_1, ReLU, conv1_2,
+ * ReLU, then the adaptation layer 1x1 conv, ReLU, 5x5 conv, eval-mode BatchNorm) followed by the sparse branch of
+ * FeatureExtractor.tensor_to_fmap: the 128-channel map of an RGB image, the size of the image, optionally L2-normalised
+ * and cast, computed by one fused kernel only where it is asked for.  Convolutions 2-4 run on tensor cores with fp16
+ * operands and fp32 accumulation; conv1_1 and the normalisation are fp32.
+ *
+ * pxr_s2dnet_weights_create uploads the weights once, in the kernel's layout.  `packed` holds n_floats = 247808 floats,
+ * each tensor in PyTorch's layout, in this order:
+ *   conv1_1 weight [64][3][3][3], bias [64]; conv1_2 weight [64][64][3][3], bias [64];
+ *   1x1 weight [64][64][1][1], bias [64]; 5x5 weight [128][64][5][5], bias [128], both with the BatchNorm folded in.
+ * A weight that is not finite, or one of layers 2-4 outside the fp16 range, is PXR_ERR_INVALID_ARGUMENT.  The weights
+ * belong to the context's device; pxr_s2dnet_weights_destroy frees them (NULL is a no-op). */
+typedef struct pxr_s2dnet_weights pxr_s2dnet_weights;
+int pxr_s2dnet_weights_create(pxr_ctx* ctx, const float* packed, int64_t n_floats, pxr_s2dnet_weights** out);
+void pxr_s2dnet_weights_destroy(pxr_s2dnet_weights* weights);
+
+/*  image      [height][width][3] uint8 RGB, host or device memory
+ *  corners    host [n][2] (x0, y0), every window inside the image: the slab [n][ps][ps][128]; NULL: the whole map
+ *             [height][width][128] (n_patches and patch_size are ignored).  A window of the slab is bit for bit the same
+ *             window of the map, and does not depend on the other windows of the call.
+ *  out_host / out_device as for pxr_extract_patches.  Every argument is checked before anything is launched.
+ *  PXR_ERR_NUMERIC: an intermediate activation is not finite in fp16 (|x| > 65504); no features are returned. */
+int pxr_s2dnet(pxr_ctx* ctx, const pxr_s2dnet_weights* weights, const uint8_t* image, int32_t image_on_device,
+               int32_t height, int32_t width, const int32_t* corners, int64_t n_patches, int32_t patch_size,
+               int32_t l2_normalize, int32_t out_dtype, void* out_host, void** out_device);
+
 /* ---- featuremetric KA ---------------------------------------------------
  * replaces _keypoint_adjustment.FeatureMetricKeypointOptimizer.run
  * (keypoint_adjustment/bindings.cc:17-34; featuremetric_keypoint_optimizer.h:50-202;

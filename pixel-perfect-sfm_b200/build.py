@@ -6,7 +6,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["pxr_api.cu", "pxr_upload.cu", "pxr_ba.cu", "pxr_ba_block.cu", "pxr_refs.cu", "pxr_ka.cu", "pxr_synth.cu", "pxr_extract.cu", "pxr_dsift.cu", "pxr_problem.cu", "pxr_qba.cu", "pxr_pnp.cu", "pxr_tri.cu"]
+SOURCES = ["pxr_api.cu", "pxr_upload.cu", "pxr_ba.cu", "pxr_ba_block.cu", "pxr_refs.cu", "pxr_ka.cu", "pxr_synth.cu", "pxr_extract.cu", "pxr_dsift.cu", "pxr_s2dnet.cu", "pxr_problem.cu", "pxr_qba.cu", "pxr_pnp.cu", "pxr_tri.cu"]
 # absolute pose estimation evaluates P3P and its residuals exactly as written, so that a host restatement in IEEE
 # double reproduces them bit for bit (tests/pnp_reference.py)
 FILE_FLAGS = {"pxr_pnp.cu": ["--fmad=false"]}

@@ -621,6 +621,65 @@ def dsift(image, corners=None, patch_size=16, num_ang_bins=8, num_spatial_bins=4
     return out if to_host else DeviceSlab(dptr.value or 0, out_shape, out_dtype, ctx)
 
 
+
+S2DNET_FLOATS = 64 * 27 + 64 + 64 * 64 * 9 + 64 + 64 * 64 + 64 + 128 * 64 * 25 + 128
+
+
+class S2DNetWeights:
+    """pxr_s2dnet_weights: S2DNet's four layers uploaded once in the kernel's layout; freed with the object"""
+
+    def __init__(self, handle, ctx):
+        self.handle, self._ctx = handle, ctx
+
+    def __del__(self):
+        try:
+            if self.handle:
+                self._ctx.lib.pxr_s2dnet_weights_destroy(C.c_void_p(self.handle))
+                self.handle = 0
+        except Exception:      # interpreter shutdown
+            pass
+
+
+def s2dnet_weights(packed, ctx=None):
+    """pxr_s2dnet_weights_create: `packed` is the S2DNET_FLOATS float32 values of include/pxr.h (conv1_1, conv1_2, 1x1 and
+    5x5 weight and bias in PyTorch's layouts, the BatchNorm folded into the last) -> S2DNetWeights"""
+    ctx = ctx or _capi.default_context()
+    packed = np.ascontiguousarray(packed, np.float32).ravel()
+    handle = C.c_void_p()
+    _capi.check(ctx.lib.pxr_s2dnet_weights_create(ctx.handle, _p(packed), C.c_int64(packed.size), C.byref(handle)))
+    return S2DNetWeights(handle.value, ctx)
+
+
+def s2dnet(image, weights, corners=None, patch_size=16, l2_normalize=True, out_dtype=np.float16, to_host=False, ctx=None):
+    """pxr_s2dnet: S2DNet features of ONE [H,W,3] uint8 RGB image (a host numpy array or anything with
+    __cuda_array_interface__).  With `corners` [n,2] (x0, y0) -> the windows [n, ps, ps, 128]; without -> the whole map
+    [1, H, W, 128].  A DeviceSlab, or a numpy array with to_host=True."""
+    ctx = ctx or _capi.default_context()
+    cai = getattr(image, "__cuda_array_interface__", None)
+    if cai is not None:
+        if cai.get("strides") is not None:
+            raise ValueError("the image must be contiguous")
+        shape, in_dtype, ptr, on_dev = tuple(cai["shape"]), np.dtype(cai["typestr"]), int(cai["data"][0]), 1
+    else:
+        image = np.ascontiguousarray(image)
+        shape, in_dtype, ptr, on_dev = image.shape, image.dtype, image.ctypes.data, 0
+    if len(shape) != 3 or shape[2] != 3 or in_dtype != np.uint8 or np.dtype(out_dtype) not in _capi.DTYPE_IDS:
+        raise ValueError("an image is a [H,W,3] uint8 array and the output float16/32/64")
+    h, w = shape[:2]
+    if corners is None:
+        out_shape, c_corners, n = (1, h, w, 128), None, 0
+    else:
+        c_corners = np.ascontiguousarray(corners, np.int32).reshape(-1, 2)
+        n = len(c_corners)
+        out_shape = (n, patch_size, patch_size, 128)
+    out = np.zeros(out_shape, out_dtype) if to_host else None
+    dptr = C.c_void_p()
+    _capi.check(ctx.lib.pxr_s2dnet(ctx.handle, C.c_void_p(weights.handle), C.c_void_p(ptr), on_dev, int(h), int(w),
+                                   _p(c_corners), C.c_int64(n), int(patch_size), int(bool(l2_normalize)),
+                                   _capi.DTYPE_IDS[np.dtype(out_dtype)], _p(out) if to_host else None,
+                                   None if to_host else C.byref(dptr)))
+    return out if to_host else DeviceSlab(dptr.value or 0, out_shape, out_dtype, ctx)
+
 def interpolate_patches(patches, corners, scales, item_patch, xys, interp=None, upsampling_factor=1.0, ctx=None):
     """pxr_interpolate_descriptors: the (bicubic, optionally L2-normalised) descriptor of patch item_patch[i] of a host
     [N,H,W,C] patch array at IMAGE coordinates xys[i] -> [n_items, C] float64"""

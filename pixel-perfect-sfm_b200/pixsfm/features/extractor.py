@@ -4,8 +4,9 @@ The reference's FeatureExtractor (pixsfm/features/extractor.py) owns the CNN (S2
 `tensor_to_fmap` (:152-236): L2-normalise the C-channel map, cast it, and either keep it dense or cut one
 `patch_size` x `patch_size` patch per keypoint with `corner = clip(int(kp * scale - ps / 2), 0, [w, h] - ps - 1)`.  The CNN
 is not part of this package; the step after it is, so that any model — a callable image name -> list of [C,H,W] maps,
-finest level first — plugs into `PixSfM(conf, extractor=DenseFeatureExtractor(model, ...))`.  The one model the package
-computes itself, dense SIFT, has the reference's `FeatureExtractor(conf)`: images in, FeatureManager out."""
+finest level first — plugs into `PixSfM(conf, extractor=DenseFeatureExtractor(model, ...))`.  The models the package
+computes itself, dense SIFT and S2DNet at num_layers 1, have the reference's `FeatureExtractor(conf)`: images in,
+FeatureManager out."""
 import os
 from pathlib import Path
 
@@ -204,34 +205,35 @@ class DenseFeatureExtractor:
 
 
 class FeatureExtractor(DenseFeatureExtractor):
-    """The reference's FeatureExtractor (features/extractor.py:28-236) for the model this package computes itself, dense
-    SIFT (`model: {name: dsift}`, features/models/dsift.py).  Each image is opened with PIL, resized per pyramid scale to
-    `round(min(max_edge / max(w, h), 1) * size * scale)` with the `resize` filter and converted to grayscale ("L", what
-    torchvision's Grayscale does); each scale gives one feature level.  Sparse features come from the fused kernel at the
+    """The reference's FeatureExtractor (features/extractor.py:28-236) for the models this package computes itself: dense
+    SIFT (`model: {name: dsift}`, features/models/dsift.py) and S2DNet at num_layers 1 (`model: {name: s2dnet}`, the
+    default; features/models/s2dnet.py, from a local weights file).  Each image is opened with PIL, resized per pyramid
+    scale to `round(min(max_edge / max(w, h), 1) * size * scale)` with the `resize` filter and converted to the mode the
+    model takes: grayscale ("L", what torchvision's Grayscale does) for dsift, "RGB" for s2dnet, so grayscale and RGBA
+    files work too.  Each scale gives one feature level.  Sparse features come from the model's fused kernel at the
     keypoints' windows only, dense ones from the same kernel over the whole map.  Cache, `on_device` and the
-    sparse-or-dense rule are DenseFeatureExtractor's.  The CNN models (S2DNet, VGG) need downloaded weights and are not
-    part of this package."""
+    sparse-or-dense rule are DenseFeatureExtractor's.  VGG is not part of this package."""
     default_conf = dict(DenseFeatureExtractor.default_conf, device="auto", fast_image_load=False, max_edge=1600,
                         model={"name": "s2dnet"}, pyr_scales=[1.0], resize="LANCZOS")
     filters = ("BILINEAR", "BICUBIC", "LANCZOS")
 
     def __init__(self, conf=None):
         conf = dict(conf or {})
-        model_conf = dict(conf.get("model") or self.default_conf["model"])
+        model_conf = dict(self.default_conf["model"], **(conf.get("model") or {}))
         super().__init__(None, None, conf)
         self.conf["model"] = model_conf
-        if model_conf.get("name") != "dsift":
-            raise ValueError("dense feature model %r is not part of this package: only 'dsift' is computed here; the CNN "
-                             "models (s2dnet, vgg) need downloaded weights — pass their FeatureManager or a "
-                             "DenseFeatureExtractor around them" % (model_conf.get("name"),))
+        if model_conf.get("name") not in ("dsift", "s2dnet"):
+            raise ValueError("dense feature model %r is not part of this package: only 'dsift' and 's2dnet' are computed "
+                             "here — pass the FeatureManager of another model or a DenseFeatureExtractor around it"
+                             % (model_conf.get("name"),))
         if self.conf["device"] not in ("auto", "cuda"):
-            raise ValueError("dense SIFT runs on the GPU only (device %r)" % (self.conf["device"],))
+            raise ValueError("dense features run on the GPU only (device %r)" % (self.conf["device"],))
         if self.conf["resize"] not in self.filters:
             raise ValueError("resize must be one of %s" % (self.filters,))
         if not self.conf["pyr_scales"] or any(float(s) <= 0 for s in self.conf["pyr_scales"]):
             raise ValueError("pyr_scales must be a non-empty list of positive scales")
-        from .models import DSIFT
-        self.model = DSIFT(model_conf)
+        from .models import DSIFT, S2DNet
+        self.model = (DSIFT if model_conf["name"] == "dsift" else S2DNet)(model_conf)
         self.channels_per_level = list(self.model.output_dims) * len(self.conf["pyr_scales"])
 
     def get_scaled_image_size(self, image, pyr_scale=1.0):
@@ -239,7 +241,8 @@ class FeatureExtractor(DenseFeatureExtractor):
         return [int(round(min(self.conf["max_edge"] / max(w, h), 1) * x * pyr_scale)) for x in (w, h)]
 
     def load_image(self, path):
-        """-> ([one [h, w] uint8 grayscale image per pyramid scale], (width, height) of the file)"""
+        """-> ([one uint8 image per pyramid scale, [h, w] grayscale or [h, w, 3] RGB as the model takes it],
+        (width, height) of the file)"""
         import PIL.Image
         image = PIL.Image.open(path)
         size = image.size
@@ -249,7 +252,7 @@ class FeatureExtractor(DenseFeatureExtractor):
         for pyr_scale in self.conf["pyr_scales"]:
             resized = image.resize(tuple(self.get_scaled_image_size(image, pyr_scale)),
                                    getattr(PIL.Image, self.conf["resize"]))
-            levels.append(np.ascontiguousarray(np.asarray(resized.convert("L"), np.uint8)))
+            levels.append(np.ascontiguousarray(np.asarray(resized.convert(self.model.image_mode), np.uint8)))
         return levels, size
 
     def _image_fmaps(self, image_dir, name, kps, ids):
@@ -263,7 +266,7 @@ class FeatureExtractor(DenseFeatureExtractor):
             ids = list(range(len(kps))) if ids is None else ids
         out = []
         for image in images:
-            h, w = self.model.map_size(*image.shape)
+            h, w = self.model.map_size(*image.shape[:2])
             scale = np.array((w / size[0], h / size[1]))
             run = dict(patch_size=ps, l2_normalize=self.conf["l2_normalize"], dtype=self.conf["dtype"],
                        to_host=not self._on_device(kps))

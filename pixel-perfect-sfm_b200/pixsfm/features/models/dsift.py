@@ -7,6 +7,7 @@ from ..._pixsfm import _engine
 
 class DSIFT:
     default_conf = {"num_ang_bins": 8, "num_spatial_bins": 4, "spatial_bin_size": 4, "rootsift": True, "clipval": 0.2}
+    image_mode = "L"
 
     def __init__(self, conf=None):
         conf = dict(conf or {})

@@ -232,10 +232,9 @@ class QueryLocalizer:
                              "target_references to 'nearest' or 'robust_mean'.")
         self.query_keypoint_adjuster = QueryKeypointAdjuster(to_ctr(self.conf.QKA))
         self.query_bundle_adjuster = QueryBundleAdjuster(to_ctr(self.conf.QBA))
-        from ..refine_colmap import _model_name
-        if extractor is None and _model_name(self.conf.dense_features) == "dsift":
-            from ..features.extractor import FeatureExtractor
-            extractor = FeatureExtractor(to_ctr(self.conf.dense_features))
+        if extractor is None:
+            from ..refine_colmap import _builtin_extractor
+            extractor = _builtin_extractor(self.conf.dense_features)
         self.extractor = extractor
         self.pose_estimator = pose_estimator
         self.reference_extractor = ba.ReferenceExtractor(to_ctr(self.conf.references), to_ctr(self.conf.interpolation))

@@ -4,9 +4,11 @@ COLMAP database -> keypoint adjustment -> database, COLMAP model -> bundle adjus
 What differs from the reference, and why:
   * dense features: with `dense_features.model.name == "dsift"` (the `dsift` preset) the driver builds the package's
     own `features.extractor.FeatureExtractor`, which computes dense SIFT on the GPU, and runs from an image directory.
-    The CNN models (S2DNet, VGG) need downloaded weights and are not part of this package: for them pass an `extractor`
-    object with the reference's interface (`extract.features_from_graph` / `features_from_reconstruction` are called
-    on it) or hand the adjusters a ready `feature_manager`.  Without either the call raises — nothing is faked.
+    With the default model, S2DNet at num_layers 1, it does the same when the weights file is there: the model's
+    `checkpoint_path` is set, or the file sits at `features/models/checkpoints/s2dnet_weights.pth`.  It is never
+    downloaded.  For VGG, or S2DNet without its weights, pass an `extractor` object with the reference's interface
+    (`extract.features_from_graph` / `features_from_reconstruction` are called on it) or hand the adjusters a ready
+    `feature_manager`.  Without either the call raises — nothing is faked.
   * models are read and written by `util.colmap_model_io` (pycolmap is not installable offline); pycolmap
     reconstructions passed in by the caller work as well (duck typing, `util/colmap_types.py`).
   * configuration: dicts (or a YAML path) merged over the reference's defaults; `${..interpolation}` of the reference's
@@ -66,6 +68,27 @@ def _model_name(dense_features):
     return model.get("name") if isinstance(model, dict) else None
 
 
+def _builtin_extractor(dense_features):
+    """the package's own FeatureExtractor for a `dense_features` block: for dsift, and for s2dnet (the default model)
+    when its weights file is given or at the default place; None otherwise"""
+    name = _model_name(dense_features) or "s2dnet"
+    if name == "s2dnet":
+        from .features.models.s2dnet import DEFAULT_CHECKPOINT
+        model = dense_features.get("model") if isinstance(dense_features, dict) else None
+        if (model or {}).get("checkpoint_path") is None and not DEFAULT_CHECKPOINT.is_file():
+            return None
+    elif name != "dsift":
+        return None
+    from .features.extractor import FeatureExtractor
+    return FeatureExtractor(to_ctr(dense_features))
+
+
+def _no_extractor_hint():
+    from .features.models.s2dnet import DEFAULT_CHECKPOINT
+    return (" (S2DNet is computed here from its weights file: set dense_features.model.checkpoint_path, or put it at %s)"
+            % DEFAULT_CHECKPOINT)
+
+
 class PixSfM:
     default_conf = {
         "interpolation": interpolation_default_conf,
@@ -89,9 +112,8 @@ class PixSfM:
         for part in ("KA", "BA"):       # "${..interpolation}": the shared block unless the adjuster has its own
             if "interpolation" not in conf.get(part, {}):
                 self.conf[part]["interpolation"] = to_conf(deepcopy(interpolation))
-        if extractor is None and _model_name(self.conf["dense_features"]) == "dsift":
-            from .features.extractor import FeatureExtractor
-            extractor = FeatureExtractor(to_ctr(self.conf["dense_features"]))
+        if extractor is None:
+            extractor = _builtin_extractor(self.conf["dense_features"])
         self.extractor = extractor
         # the reference builds its extractor FROM conf.dense_features (refine_colmap.py:52-56); here the extractor comes in
         # from outside (the CNN is not part of this package), so the block is applied to it where it knows the option
@@ -105,7 +127,8 @@ class PixSfM:
     def _features(self, how, *args, cache_path=None):
         if self.extractor is None:
             raise ValueError("no feature_manager given and no extractor configured: dense feature extraction (the CNN) "
-                             "is outside this package — pass feature_manager= or PixSfM(conf, extractor=...)")
+                             "is outside this package — pass feature_manager= or PixSfM(conf, extractor=...)"
+                             + _no_extractor_hint())
         return getattr(self.extractor, how)(*args, cache_path=cache_path)
 
     # ---------------------------------------------------------------------------------------- KA

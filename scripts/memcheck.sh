@@ -3,7 +3,7 @@
 #   scripts/memcheck.sh > memcheck.log 2>&1
 # Every kernel family is touched once: K0/K1 (all dtypes), build, Schur, persistent Cholesky, PCG dense + block-sparse,
 # inner iterations, reference extraction, cost maps, KA (edge and query mode), dense SIFT, batched query BA (2 500 blocks,
-# 18 columns), triangulation (verification, RANSAC tracks, evaluation).
+# 18 columns), triangulation (verification, RANSAC tracks, evaluation), S2DNet.
 set -u
 run() {
   echo "=== $*"
@@ -15,5 +15,6 @@ run tests/test_gpu_costmaps.py -k "extraction_matches or fused or full_solve"
 run tests/test_gpu_ka.py
 run tests/test_gpu_edge_cases.py -k "triangulation or single_free or clamped"
 run tests/test_gpu_dsift.py -k "not past_2_to_the_31"
+run tests/test_gpu_s2dnet.py -k "not past_2_to_the_31"
 run tests/test_gpu_query_refinement_reference.py -k "b2500_full_opencv_all or b257_full_opencv_all"
 run tests/test_gpu_triangulation.py
